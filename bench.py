@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the stylize() hot path: iterations/sec at end_scale=2048 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--size 2048] [--impl native|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--size 2048] [--impl native|reference] [--dump-outputs DIR]
 
 A "step" is one stylize iteration (VGG-19 forward, W2/content/TV losses, backward to the image, Adam+clamp+EMA)
 on a synthetic 2048x2048 content+style pair with the seeded synthetic VGG-19 (no network for images/checkpoints).
@@ -12,11 +12,15 @@ native arm   value   = it/s of K stb_iterate calls, state resident in HBM, CUDA 
                        iterations, callback reading the loss every iteration) -- host PIL inputs, H2D of the
                        resized images, per-iteration D2H of the loss, final D2H of the result, all inside the timed
                        region (wall clock around the call, since it spans host work).
-             roofline= conv tensor-pipe: algorithmic conv FLOPs per iteration / summed duration of the tcgen05 conv
-                       launches (CUDA events around every launch, second instrumented pass), vs the measured
-                       sustained bf16 peak of MEASURED_PEAKS.json.
-             cpu_baseline = the UNMODIFIED reference (baseline/_ref; else the oracle port) timed on all host cores for one
+             roofline= conv tensor-pipe: algorithmic conv FLOPs per iteration / summed duration of the wgmma conv
+                       launches (CUDA events around every launch, second instrumented pass), vs the bf16 peak of
+                       MEASURED_PEAKS.json, else the H100 SXM data sheet's dense bf16 figure.
+             cpu_baseline = the UNMODIFIED reference (oracle/_ref; else the oracle port) timed on all host cores for one
                        real iteration at the benchmark size after a warm-up iteration (no extrapolation).
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step computed -- the image, the EMA of
+                       the image and the eight loss values -- as DIR/<name>.npy (float32, at most 64 MB in all; an array
+                       over its share is written as a fixed, seeded sample <name>_sample.npy).  The inputs depend on
+                       the arguments only, so two builds can be compared output for output.
 reference arm (--impl reference): 2-3 real 2048^2 iterations of the reference's CPU path + configs[0] (256^2, 50
                        iterations), printed in the same JSON shape.
 N > 1: ONE 2048x2048 job tiled spatially over the N GPUs (strong scaling): horizontal bands with 80-row halo aprons;
@@ -49,11 +53,27 @@ def measured_peaks():
         d = json.loads(p.read_text())
         return dict(hbm_gbs=d['hbm_gbs'], bf16_tflops=d['bf16_tflops'],
                     bf16_tflops_sustained=d.get('bf16_tflops_sustained', d['bf16_tflops']), source='measured')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source='fallback')
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- a ceiling, not a measured rate
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source='H100 SXM data sheet')
+
+
+def dump_outputs(out_dir, arrays, budget=64 << 20):
+    """Write each (name, tensor, share of the byte budget) as out_dir/<name>.npy in float32; a tensor larger than its
+    share is written as <name>_sample.npy, the elements at a fixed, seeded set of flat indices."""
+    import numpy as np
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, t, share in arrays:
+        a = t.detach().float().cpu().numpy()
+        cap = int(budget * share) // 4
+        if a.size <= cap:
+            np.save(out_dir / f'{name}.npy', a)
+        else:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, cap, replace=False))
+            np.save(out_dir / f'{name}_sample.npy', a.ravel()[idx])
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -124,8 +144,8 @@ class _Budget(Exception):
 
 
 def reference_iteration_times(size, n_iters, budget_s):
-    """Per-iteration wall times of the UNMODIFIED reference's stylize() (single scale, size x size, CPU) when its
-    install travelled with the repo (baseline/_ref), else of the oracle port of the same loop body.  Returns
+    """Per-iteration wall times of the UNMODIFIED reference's stylize() (single scale, size x size, CPU) when build()
+    copied it into oracle/_ref, else of the oracle port of the same loop body.  Returns
     (kind, [seconds per iteration, first one excluded], threads).  Stops early once budget_s is exceeded."""
     import torch
     from oracle import reference_harness as RH
@@ -279,7 +299,7 @@ def run_native(args, rank, local_rank, world):
         sampler.start()
     # ---- REPEATS timed regions of exactly `steps` iterations each (barrier + synchronize on both sides, CUDA events,
     # max over ranks per region); the reported value is the MEDIAN region, the others are listed
-    # (N = 1: the contract's single region of exactly `steps` iterations; N > 1: five, because a tiled region of ~50 ms
+    # (N = 1: a single region of exactly `steps` iterations; N > 1: five, because a tiled region of ~50 ms
     # is bimodal when any rank's host stalls)
     REPEATS = 5 if world > 1 else 1
     region_ms = []
@@ -299,6 +319,9 @@ def run_native(args, rank, local_rank, world):
     r1, k1, per_graph = m.launch_count()
     clocks = sampler.stop() if rank == 0 else None
     final_loss = float(st._loss_host[0])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), [('image', st.image, 0.75), ('average', st.average.value, 0.15),
+                                               ('loss_terms', st._loss_host, 0.05)])
     ms_total = sorted(region_ms)[len(region_ms) // 2]
     ms_per_step = ms_total / args.steps
     tiled = band is not None
@@ -361,8 +384,7 @@ def run_native(args, rank, local_rank, world):
     with contextlib.redirect_stdout(io.StringIO()):  # stylize() prints progress like the reference does
         st2.stylize(content, [style], min_scale=size, end_scale=size, initial_iterations=2, callback=lambda it: None)
     barrier()
-    # BASELINE.json's config runs 500 iterations at this scale; fewer would mostly time the per-call setup
-    e2e_its = max(args.steps, 500)
+    e2e_its = args.steps
     t0 = time.perf_counter()
     with contextlib.redirect_stdout(io.StringIO()):
         out = st2.stylize(content, [style], min_scale=size, end_scale=size, initial_iterations=e2e_its,
@@ -379,7 +401,7 @@ def run_native(args, rank, local_rank, world):
     e2e = dict(value=e2e_its / t_e2e, unit='it/s', h2d_bytes_per_step=h2d / e2e_its,
                d2h_bytes_per_step=d2h / e2e_its, iterations=e2e_its,
                note='StyleTransfer.stylize(PIL inputs, single scale, per-iteration loss callback) wall clock over '
-                    f'{e2e_its} iterations (BASELINE.json config: 500 at this scale), incl. PIL resize, target '
+                    f'{e2e_its} iterations, incl. PIL resize, target '
                     'extraction, H2D of the inputs, per-iteration loss D2H, final image D2H')
 
     if rank == 0:
@@ -390,18 +412,10 @@ def run_native(args, rank, local_rank, world):
         conv_ms = prof['conv_fwd']['ms_per_iter'] + prof['conv_bwd']['ms_per_iter']
         achieved = conv_flops / (conv_ms / 1000.0) / 1e12
         peak = peaks['bf16_tflops_sustained']
-        traffic, traffic_src = None, None
-        for cand in ('r2_conv_traffic.json', 'r1_conv_traffic.json'):
-            tpath = ROOT / 'profiles' / cand
-            if tpath.exists() and size == 2048 and world == 1:
-                traffic = json.loads(tpath.read_text())['dram_total_bytes']  # dram read+write of the conv launches, ncu
-                traffic_src = f'profiles/{cand} (one ncu --set full capture of the same command; not measured in this run)'
-                break
         roofline = dict(bound='tensor', achieved=achieved, peak=peak, unit='TFLOP/s', frac=achieved / peak,
-                        traffic=traffic, traffic_source=traffic_src,
                         peak_source=f"{peaks['source']} (bf16_tflops_sustained)",
                         frac_of_burst_peak=achieved / peaks['bf16_tflops'],
-                        kernel='pixel_gemm_kernel (tcgen05 conv fwd+dgrad incl. tap-gradient GEMMs, 25 launches/iter)',
+                        kernel='pixel_gemm_kernel (wgmma conv fwd+dgrad incl. tap-gradient GEMMs, 25 launches/iter)',
                         note='algorithmic FLOPs/iter of the twelve 3x3 convs (1437696/pixel) / summed CUDA-event duration of the conv '
                              'launches in an instrumented pass of this run',
                         step_fraction=conv_ms / sum(v['ms_per_iter'] for v in prof.values()),
@@ -427,7 +441,7 @@ def run_native(args, rank, local_rank, world):
                     config=dict(workload=f'{size}x{size} single scale (BASELINE.json configs[2]), pooling=max, '
                                          'content+1 style, bf16 operands / fp32 accumulate, fp32 sqrtm+Adam',
                                 parallelism=par,
-                                l2='working set per iteration (>= 2.4 GB of activations) far exceeds the 126 MB L2',
+                                l2='working set per iteration (>= 2.4 GB of activations) far exceeds the 50 MB L2',
                                 final_loss=final_loss,
                                 timing=(f'median of {REPEATS} timed regions of {args.steps} iterations each' if REPEATS > 1 else
                                         f'one timed region of {args.steps} iterations'),
@@ -454,6 +468,7 @@ def main():
     ap.add_argument('--size', type=int, default=2048)
     ap.add_argument('--impl', default='native', choices=['native', 'reference'])
     ap.add_argument('--no-cpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None)
     args = ap.parse_args()
     rank = int(os.environ.get('RANK', '0'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))

@@ -1,4 +1,4 @@
-/* libstb200 -- C ABI of the B200-native stylize() hot path.
+/* libstb200 -- C ABI of the H100-native stylize() hot path.
  *
  * The reference (crowsonkb/style-transfer-pytorch) has no FFI layer: its hot path is the Python loop body of
  * StyleTransfer.stylize() (style_transfer/style_transfer.py:472-486, "ST" below).  This header is the seam a

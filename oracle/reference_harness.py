@@ -1,10 +1,10 @@
 """TEST / BASELINE INFRASTRUCTURE ONLY -- runs the UNMODIFIED reference with the synthetic VGG fixture.
 
-The reference tree is looked up at /root/reference (build container) and then at baseline/_ref (a git-ignored
-`pip install --no-deps --target baseline/_ref` of the same unmodified sources, which travels to the GPU box).  Used by
-tests/golden/make_golden.py to produce the committed golden vectors that pin oracle/st_oracle.py, by tests that are
-skipped when the reference is absent, and by bench.py's reference arm / cpu_baseline leg.  The only thing patched is
-torchvision's checkpoint *download* (no network here): the reference code itself runs untouched.
+The reference modules are looked up in oracle/_ref (git-ignored; `build()` copies them there from a reference checkout
+when one is present: oracle/Makefile's default location or STB_REFERENCE_DIR).  Used by tests/golden/make_golden.py to produce the committed golden vectors that pin
+oracle/st_oracle.py, by tests that are skipped when the reference is absent, and by bench.py's reference arm /
+cpu_baseline leg.  The only thing patched is torchvision's checkpoint *download* (no network needed): the reference
+code itself runs untouched.
 """
 from __future__ import annotations
 
@@ -15,8 +15,7 @@ from pathlib import Path
 
 import torch
 
-_CANDIDATES = [Path('/root/reference'), Path(__file__).resolve().parent.parent / 'baseline' / '_ref']
-REFERENCE_ROOT = next((c for c in _CANDIDATES if (c / 'style_transfer' / 'style_transfer.py').exists()), _CANDIDATES[0])
+REFERENCE_ROOT = Path(__file__).resolve().parent / '_ref'
 
 
 def reference_available() -> bool:
@@ -52,7 +51,7 @@ def patched_checkpoint(conv_weights):
 
 def import_reference():
     """Import the reference's style_transfer.style_transfer module without its package __init__ (which pulls the
-    aiohttp web UI); the module itself is loaded from the read-only tree, unmodified."""
+    aiohttp web UI); the module itself is loaded unmodified."""
     import importlib.util
     import types
     name = 'ref_style_transfer'

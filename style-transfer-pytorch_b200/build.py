@@ -1,7 +1,7 @@
-"""In-tree build of libstb200.so (the C-ABI CUDA library) with nvcc for sm_100a.
+"""In-tree build of libstb200.so (the C-ABI CUDA library) with nvcc for sm_90a (H100).
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot; there is no JIT and no fallback:
-if the library is missing, loading it raises.
+The .so is a git-ignored build product next to this file; there is no JIT and no fallback: if the library is
+missing, loading it raises.
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ TEST_ONLY_SOURCES = {'api_test.cu'}
 OBJ_DIR = PKG_DIR / 'build'
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
     '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '-cudart', 'static',
     f'-I{INCLUDE}', f'-I{CSRC}',
 ]
@@ -47,7 +47,7 @@ def _stale() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every csrc/*.cu for sm_100a; link libstb200.so (product: everything but the test hooks) and
+    """Compile every csrc/*.cu for sm_90a; link libstb200.so (product: everything but the test hooks) and
     libstb200_test.so (the same objects + api_test.o, loaded by tests/ only) next to this file."""
     if not force and not _stale():
         return LIB_PATH

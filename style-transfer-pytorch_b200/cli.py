@@ -1,4 +1,4 @@
-"""`style_transfer` console entry point for the B200-native build.
+"""`style_transfer` console entry point for the H100-native build.
 
 Same flags as the reference CLI (/root/reference/style_transfer/cli.py:155-203): positional content + styles,
 `-o/--output`, `-sw/--style-weights`, `-d/--devices`, `-r/--random-seed`, `-p/--pooling`, `--save-every`, and one
@@ -63,7 +63,7 @@ def build_parser():
 def main(argv=None):
     args = build_parser().parse_args(argv)
     if args.web or args.proof:
-        sys.exit('--web / --proof are outside the scope of the B200-native hot-path build')
+        sys.exit('--web / --proof are outside the scope of the H100-native hot-path build')
     out_path = Path(args.output)
     if out_path.suffix.lower() in ('.tif', '.tiff'):
         sys.exit('16-bit TIFF output is outside the scope of this build; use .png/.jpg/.webp')

@@ -1,7 +1,7 @@
-// C-ABI of the B200-native stylize() hot path (see include/stb200.h).  The context owns an explicit, static
+// C-ABI of the H100-native stylize() hot path (see include/stb200.h).  The context owns an explicit, static
 // forward/backward schedule for torchvision vgg19().features[:30] -- no autograd on the path:
-//   forward   ST:78-90     conv0 (+TV) -> 12 x tcgen05 conv/bias/ReLU, 4 pools, taps 1,6,11,20,22,29
-//   losses    ST:119-126, 149-181, 184-195, 198-234  content MSE, 5 x W2 style (Gram on tcgen05, sqrtm in fp32), TV
+//   forward   ST:78-90     conv0 (+TV) -> 12 x wgmma conv/bias/ReLU, 4 pools, taps 1,6,11,20,22,29
+//   losses    ST:119-126, 149-181, 184-195, 198-234  content MSE, 5 x W2 style (Gram on wgmma, sqrtm in fp32), TV
 //   backward  ST:475       tap-gradient GEMMs folded into the dgrad chain, pool backward, conv0 dgrad
 //   update    ST:481-486   Adam + clamp + EMA fused into the last kernel
 #include <cmath>
@@ -908,7 +908,7 @@ int stb_adam_update(float* img, const float* grad, float* exp_avg, float* exp_av
   const AdamScalars as = make_adam_scalars(step, lr, beta1, beta2, adam_eps, ema_decay);
   const long n = 3l * rows * W;
   long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 16l * num_sms()) blocks = 16l * num_sms();
   adam_rows_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, grad, exp_avg, exp_avg_sq, ema, H,
                                                                                   W, row0, rows, as);
   STB_CUDA_CHECK(cudaGetLastError());

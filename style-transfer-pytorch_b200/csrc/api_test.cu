@@ -42,7 +42,7 @@ extern "C" {
 
 int stb_test_conv0_fwd(const float* img, const float* w0, const float* b0, void* out_bf16, int H, int W,
                        float tv_weight, float* gtv, float* tv_partials, int* n_partials, void* stream) {
-  // product path of conv0: TV kernel and the fused im2col + tcgen05 GEMM + bias + ReLU kernel
+  // product path of conv0: TV kernel and the fused im2col + wgmma GEMM + bias + ReLU kernel
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (gtv != nullptr) STB_TRY(launch_tv(img, H, W, 0, H, H, tv_weight, gtv, tv_partials, n_partials, s));
   bf16* wp = nullptr;
@@ -56,7 +56,7 @@ int stb_test_conv0_fwd(const float* img, const float* w0, const float* b0, void*
 
 int stb_test_conv0_bwd(const void* g0_bf16, const float* w0, const float* gtv, float* grad_out, int H, int W,
                        void* stream) {
-  // product path: interior via the tcgen05 1x1 GEMM + col2im kernel with the image-space epilogue, borders in SIMT
+  // product path: interior via the wgmma 1x1 GEMM + col2im kernel with the image-space epilogue, borders in SIMT
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   bf16* wp = nullptr;
   STB_CUDA_CHECK(cudaMalloc(&wp, 32 * 64 * 2));

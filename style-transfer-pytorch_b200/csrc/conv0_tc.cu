@@ -1,5 +1,5 @@
-// conv0 forward (Normalize + replicate-pad 3x3 conv 3 -> 64 + bias + ReLU) as ONE tcgen05 kernel:
-//   VGGFeatures.forward, first module    /root/reference/style_transfer/style_transfer.py:39,52-59,85-89  (ST)
+// conv0 forward (Normalize + replicate-pad 3x3 conv 3 -> 64 + bias + ReLU) as ONE wgmma kernel:
+//   VGGFeatures.forward, first module    style_transfer/style_transfer.py:39,52-59,85-89 of the reference  (ST)
 //   transforms.Normalize                 ST:30-31
 // K = 27 is too short for a tensor-core GEMM and fp32 pixels do not fit bf16, so every pixel's K row is the im2col of
 // the normalised, replicate-padded image in split form: k < 27 the bf16 "hi" part of tap (c*3+ky)*3+kx, 27 <= k < 54
@@ -9,10 +9,10 @@
 // traffic left is the 12 B/pixel image read and the 128 B/pixel activation write, which is the bound.
 //
 // Persistent CTAs (two per SM: the roles are latency- not throughput-bound).  Work item = 4 image rows x 128 pixels (4 M-tiles sharing one 6 x 130 x 3 halo):
-//   warps 1-8  producers: halo via cp.async (next item prefetched during the current one), one thread per pixel
-//              builds the 128-byte K row, fence.proxy.async, arrive on the tile's "full" mbarrier
-//   warp 0     tcgen05.mma issuer: 4 x (M128 N64 K16) per tile into a ring of 2 TMEM accumulators
-//   warps 9-12 epilogue: tcgen05.ld -> + bias, ReLU -> bf16 -> swizzled staging -> TMA store (OOB pixels clipped)
+//   warps 4-11 producers: halo via cp.async (next item prefetched during the current one), one thread per pixel
+//              builds the 128-byte K row, fence.proxy.async, arrive on the tile's "full" mbarrier (ring of 2 tiles)
+//   warps 0-3  one warpgroup: 2 x 4 x wgmma (M64 N64 K16) per tile into registers, one M64 half at a time -> + bias, ReLU -> bf16 ->
+//              swizzled staging -> TMA store (OOB pixels clipped)
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -21,9 +21,9 @@ namespace stb {
 namespace {
 
 constexpr int C0_PX = 128, C0_ROWS = 4;
-constexpr int C0_RING = 2;                          // A tiles in flight = TMEM accumulators
+constexpr int C0_RING = 2;                          // A tiles in flight
 constexpr int C0_PROD = 256, C0_EPI = 128;
-constexpr int C0_THREADS = 32 + C0_PROD + C0_EPI;   // 416
+constexpr int C0_THREADS = C0_EPI + C0_PROD;        // 384
 constexpr int HALO_W = 132, HALO_ROWS = C0_ROWS + 2;
 constexpr int HALO_FLOATS = 3 * HALO_ROWS * HALO_W;
 constexpr int A_TILE = C0_PX * 128;                 // 16 KiB
@@ -33,8 +33,7 @@ constexpr int OFF_STG = OFF_B + 64 * 128;           // 2 x 16 KiB store staging
 constexpr int OFF_HALO = OFF_STG + 2 * A_TILE;
 constexpr int OFF_BIAS = OFF_HALO + 2 * HALO_FLOATS * 4;
 constexpr int OFF_BAR = OFF_BIAS + 64 * 4;
-constexpr int OFF_TMEM = OFF_BAR + 4 * C0_RING * 8;
-constexpr int C0_SMEM = OFF_TMEM + 16 + 1024;
+constexpr int C0_SMEM = OFF_BAR + 2 * C0_RING * 8 + 1024;
 static_assert(OFF_HALO % 16 == 0 && OFF_BAR % 8 == 0, "alignment");
 
 __constant__ float c0_mean[3] = {0.485f, 0.456f, 0.406f};
@@ -53,9 +52,6 @@ conv0_fwd_kernel(const float* __restrict__ img, const bf16* __restrict__ w0p, co
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* a_empty = a_full + C0_RING;
-  uint64_t* t_full = a_empty + C0_RING;
-  uint64_t* t_empty = t_full + C0_RING;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + OFF_TMEM);
   float* s_bias = reinterpret_cast<float*>(smem + OFF_BIAS);
   float* s_halo = reinterpret_cast<float*>(smem + OFF_HALO);
 
@@ -66,14 +62,11 @@ conv0_fwd_kernel(const float* __restrict__ img, const bf16* __restrict__ w0p, co
   if (threadIdx.x == 0) {
     for (int i = 0; i < C0_RING; ++i) {
       mbar_init(&a_full[i], C0_PX);
-      mbar_init(&a_empty[i], 1);
-      mbar_init(&t_full[i], 1);
-      mbar_init(&t_empty[i], C0_EPI);
+      mbar_init(&a_empty[i], 4);   // one arrival per MMA warp once its wgmma reads are complete
     }
     fence_barrier_init();
     tma_prefetch_desc(&tm_out);
   }
-  if (warp == 0) tmem_alloc<C0_RING * 64>(tmem_ptr);
   // weights -> SW128 K-major tile, bias
   for (int i = threadIdx.x; i < 512; i += C0_THREADS) {
     const int n = i >> 3, j = i & 7;
@@ -82,41 +75,60 @@ conv0_fwd_kernel(const float* __restrict__ img, const bf16* __restrict__ w0p, co
   }
   if (threadIdx.x < 64) s_bias[threadIdx.x] = bias[threadIdx.x];
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(128, 64, 0, 0);
-    constexpr uint32_t dhi = umma_desc_hi_sw128(1024);
-    const bool leader = elect_one();
-    const uint32_t b_lo = umma_desc_lo(smem_u32(smem + OFF_B));
+  if (warp < 4) {
+    // ------------------------------------------------------------------ MMA + epilogue warpgroup
+    const int te = threadIdx.x;
+    const int cq = 2 * (lane & 3);
+    const uint64_t bd = gmma_desc_k(smem_u32(smem + OFF_B));
     uint32_t tc = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int y0 = (item / items_x) * C0_ROWS;
+      const int y0 = (item / items_x) * C0_ROWS, x0 = (item % items_x) * C0_PX;
       const int nt = min(C0_ROWS, H - y0);
       for (int r = 0; r < nt; ++r, ++tc) {
         const int slot = tc & (C0_RING - 1);
-        const uint32_t ph = (tc / C0_RING) & 1;
-        mbar_wait(&a_full[slot], ph);
-        mbar_wait(&t_empty[slot], ph ^ 1);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t a_lo = umma_desc_lo(smem_u32(smem + OFF_A + slot * A_TILE));
+        mbar_wait(&a_full[slot], (tc / C0_RING) & 1);
+        const uint32_t a_tile = smem_u32(smem + OFF_A + slot * A_TILE);
+        uint8_t* stg = smem + OFF_STG + (tc & 1) * A_TILE;
+        if (te == 0) tma_store_wait_read<1>();  // the store issued two tiles ago has drained this buffer
+        named_bar_sync(3, C0_EPI);
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_split(tmem_base + slot * 64, a_lo + 2 * k, dhi, b_lo + 2 * k, dhi, idesc, k > 0);
-          umma_commit(&a_empty[slot]);
-          umma_commit(&t_full[slot]);
+        for (int h = 0; h < 2; ++h) {   // pixels 64 h .. 64 h + 63, one after the other (32 accumulator registers)
+          float acc[32];
+          const uint64_t ad = gmma_desc_k(a_tile + h * 64 * 128);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_bf16<0, 0>(acc, ad + 2 * k, bd + 2 * k, k > 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_acc(acc);
+          if (h == 1 && lane == 0) mbar_arrive(&a_empty[slot]);
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int p = 64 * h + 16 * warp + (lane >> 2) + 8 * half;  // pixel of the tile
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+              const int n = 8 * q + cq;
+              const float a = acc[4 * q + 2 * half] + s_bias[n];
+              const float b = acc[4 * q + 2 * half + 1] + s_bias[n + 1];
+              *reinterpret_cast<uint32_t*>(stg + p * 128 + ((q ^ (p & 7)) << 4) + cq * 2) =
+                  pack_bf16x2(fmaxf(a, 0.f), fmaxf(b, 0.f));
+            }
+          }
         }
-        __syncwarp();
+        fence_proxy_async_smem();
+        named_bar_sync(3, C0_EPI);
+        if (te == 0) {
+          tma_store_3d(&tm_out, stg, 0, x0, y0 + r);
+          tma_store_commit();
+        }
       }
     }
-  } else if (warp <= C0_PROD / 32) {
+    if (te == 0) tma_store_wait_all0();
+  } else {
     // ------------------------------------------------------------------ producers
-    const int tp = threadIdx.x - 32;
+    const int tp = threadIdx.x - C0_EPI;
     const int half = tp >> 7, x = tp & (C0_PX - 1);
     const float inv_std[3] = {(float)(1.0 / 0.229), (float)(1.0 / 0.224), (float)(1.0 / 0.225)};
     auto prefetch = [&](int item, int buf) {
@@ -172,83 +184,30 @@ conv0_fwd_kernel(const float* __restrict__ img, const bf16* __restrict__ w0p, co
       }
       tc += nt;
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue
-    const int wq = warp & 3;
-    const int p = wq * 32 + lane;  // TMEM lane = pixel of the tile
-    const int te = threadIdx.x - 32 - C0_PROD;
-    uint32_t tc = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int y0 = (item / items_x) * C0_ROWS, x0 = (item % items_x) * C0_PX;
-      const int nt = min(C0_ROWS, H - y0);
-      for (int r = 0; r < nt; ++r, ++tc) {
-        const int slot = tc & (C0_RING - 1);
-        mbar_wait(&t_full[slot], (tc / C0_RING) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + slot * 64 + (static_cast<uint32_t>(wq * 32) << 16);
-        uint8_t* stg = smem + OFF_STG + (tc & 1) * A_TILE;
-        if (te == 0) tma_store_wait_read<1>();  // the store issued two tiles ago has drained this buffer
-        named_bar_sync(3, C0_EPI);
-        uint8_t* row = stg + p * 128;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t v[32];
-          tmem_ld_32x32(taddr + 32 * h, v);
-          tmem_ld_wait();
-          if (h == 1) {  // accumulator fully read: hand it back to the MMA warp
-            tc_fence_before();
-            mbar_arrive(&t_empty[slot]);
-          }
-#pragma unroll
-          for (int ch = 0; ch < 4; ++ch) {
-            uint32_t wv[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int n = 8 * ch + 2 * q;
-              const float a = __uint_as_float(v[n]) + s_bias[32 * h + n];
-              const float b = __uint_as_float(v[n + 1]) + s_bias[32 * h + n + 1];
-              wv[q] = pack_bf16x2(fmaxf(a, 0.f), fmaxf(b, 0.f));
-            }
-            *reinterpret_cast<uint4*>(row + (((4 * h + ch) ^ (p & 7)) << 4)) = make_uint4(wv[0], wv[1], wv[2], wv[3]);
-          }
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(3, C0_EPI);
-        if (te == 0) {
-          tma_store_3d(&tm_out, stg, 0, x0, y0 + r);
-          tma_store_commit();
-        }
-      }
-    }
-    if (te == 0) tma_store_wait_all0();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<C0_RING * 64>(tmem_base);
 }
 
 
 // =====================================================================================================================
 // conv0 backward for the interior pixels + the optimiser step, as a 1x1 GEMM followed by a 3x3 "col2im" in shared
 // memory (autograd of ST:85-89 w.r.t. the image, then ST:481-486):
-//     D[p][(ky,kx,c)] = sum_co g0[p][co] * w0[co][c][ky][kx]            tcgen05, M = 128 pixels, N = 32 (27 used), K = 64
+//     D[p][(ky,kx,c)] = sum_co g0[p][co] * w0[co][c][ky][kx]            wgmma, M = 128 pixels, N = 32 (27 used), K = 64
 //     grad[c][y][x]   = sum_{ky,kx} D[(y-ky+1, x-kx+1)][(ky,kx,c)]      27 shared-memory reads per pixel
 // A direct dgrad GEMM (K = 9 x 64, N = 3 padded to 16) re-reads every g0 pixel from shared memory nine times and was
 // shared-memory-bandwidth bound at 2.5x the HBM time; here every g0 row is loaded and multiplied exactly once.
 // Work item = a vertical strip: 126 output columns (128 D columns incl. the one-pixel halo) x 32 output rows (34 D
-// rows).  Roles: warp 0 TMA producer (one 128-pixel g0 row per stage, zero-filled outside the image = the conv's zero
-// padding), warp 1 MMA issuer (ring of 2 TMEM accumulators; two CTAs per SM), warps 2-5: accumulator row -> D ring (4 rows, k-major
-// planes) -> gather for the output row one above -> Normalize backward + TV gradient + Adam + clamp + EMA with fully
-// coalesced accesses to the fp32 planes, whose loads are issued one row ahead.
+// rows).  Roles: warp 4 TMA producer (ring of 2 stages of one 128-pixel g0 row each, zero-filled outside the image = the
+// conv's zero padding; two CTAs per SM), warps 0-3 one warpgroup: wgmma of the row into registers -> D ring (4 rows,
+// k-major planes) -> gather for the output row one above -> Normalize backward + TV gradient + Adam + clamp + EMA with
+// fully coalesced accesses to the fp32 planes, whose loads are issued one row ahead.
 constexpr int BW_OUT = 126, BW_ROWS = 32, BW_RING = 2;
-constexpr int BW_THREADS = 64 + 128;
+constexpr int BW_THREADS = 128 + 32;
 constexpr int D_PITCH = 132, D_SLOT = 27 * D_PITCH;   // floats
 constexpr int BW_OFF_A = 0;
 constexpr int BW_OFF_B = BW_OFF_A + BW_RING * A_TILE;  // 32 x 128 B weights
 constexpr int BW_OFF_D = BW_OFF_B + 32 * 128;
 constexpr int BW_OFF_BAR = BW_OFF_D + 4 * D_SLOT * 4;
-constexpr int BW_OFF_TMEM = BW_OFF_BAR + 4 * BW_RING * 8;
-constexpr int BW_SMEM = BW_OFF_TMEM + 16 + 1024;
+constexpr int BW_SMEM = BW_OFF_BAR + 2 * BW_RING * 8 + 1024;
 static_assert(BW_OFF_BAR % 8 == 0, "alignment");
 
 struct ImgState {
@@ -264,9 +223,6 @@ conv0_bwd_kernel(const __grid_constant__ CUtensorMap tm_g0, const bf16* __restri
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + BW_OFF_BAR);
   uint64_t* a_empty = a_full + BW_RING;
-  uint64_t* t_full = a_empty + BW_RING;
-  uint64_t* t_empty = t_full + BW_RING;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + BW_OFF_TMEM);
   float* s_d = reinterpret_cast<float*>(smem + BW_OFF_D);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -276,26 +232,20 @@ conv0_bwd_kernel(const __grid_constant__ CUtensorMap tm_g0, const bf16* __restri
   if (threadIdx.x == 0) {
     for (int i = 0; i < BW_RING; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-      mbar_init(&t_full[i], 1);
-      mbar_init(&t_empty[i], 128);
+      mbar_init(&a_empty[i], 4);   // one arrival per MMA warp once its wgmma reads are complete
     }
     fence_barrier_init();
     tma_prefetch_desc(&tm_g0);
   }
-  if (warp == 1) tmem_alloc<BW_RING * 32>(tmem_ptr);
   for (int i = threadIdx.x; i < 256; i += BW_THREADS) {  // weights [32 n][64 co] -> SW128 K-major tile
     const int n = i >> 3, j = i & 7;
     *reinterpret_cast<uint4*>(smem + BW_OFF_B + n * 128 + ((j ^ (n & 7)) << 4)) =
         *reinterpret_cast<const uint4*>(w0q + n * 64 + j * 8);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       uint32_t tc = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -310,35 +260,10 @@ conv0_bwd_kernel(const __grid_constant__ CUtensorMap tm_g0, const bf16* __restri
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = umma_idesc_bf16(128, 32, 0, 0);
-    constexpr uint32_t dhi = umma_desc_hi_sw128(1024);
-    const bool leader = elect_one();
-    const uint32_t b_lo = umma_desc_lo(smem_u32(smem + BW_OFF_B));
-    uint32_t tc = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int ys = (item / strips) * BW_ROWS;
-      const int nd = min(BW_ROWS, H - ys) + 2;
-      for (int j = 0; j < nd; ++j, ++tc) {
-        const int slot = tc & (BW_RING - 1);
-        const uint32_t ph = (tc / BW_RING) & 1;
-        mbar_wait(&a_full[slot], ph);
-        mbar_wait(&t_empty[slot], ph ^ 1);
-        tc_fence_after();
-        if (leader) {
-          const uint32_t a_lo = umma_desc_lo(smem_u32(smem + BW_OFF_A + slot * A_TILE));
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_split(tmem_base + slot * 32, a_lo + 2 * k, dhi, b_lo + 2 * k, dhi, idesc, k > 0);
-          umma_commit(&a_empty[slot]);
-          umma_commit(&t_full[slot]);
-        }
-        __syncwarp();
-      }
-    }
   } else {
-    const int wq = warp & 3;
-    const int t = wq * 32 + lane;  // TMEM lane = D column of the strip; output column for 1 <= t <= 126
+    const int t = threadIdx.x;     // D column of the strip in the gather; output column for 1 <= t <= 126
+    const int cq = 2 * (lane & 3);
+    const uint64_t bd = gmma_desc_k(smem_u32(smem + BW_OFF_B));
     AdamScalars ac{};
     if (apply_update) ac = *adam;
     const float inv_std[3] = {(float)(1.0 / 0.229), (float)(1.0 / 0.224), (float)(1.0 / 0.225)};
@@ -365,16 +290,35 @@ conv0_bwd_kernel(const __grid_constant__ CUtensorMap tm_g0, const bf16* __restri
       for (int j = 0; j < nd; ++j, ++tc) {
         if (j + 1 >= 2 && j + 1 < nd) load_state(ys + j - 1, nxt);  // state of the NEXT iteration's output row
         const int slot = tc & (BW_RING - 1);
-        mbar_wait(&t_full[slot], (tc / BW_RING) & 1);
-        tc_fence_after();
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + slot * 32 + (static_cast<uint32_t>(wq * 32) << 16), v);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(&t_empty[slot]);
+        mbar_wait(&a_full[slot], (tc / BW_RING) & 1);
+        float acc[2][16];
+        const uint32_t a_tile = smem_u32(smem + BW_OFF_A + slot * A_TILE);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {   // D columns 64 h .. 64 h + 63
+          const uint64_t ad = gmma_desc_k(a_tile + h * 64 * 128);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_bf16<0, 0>(acc[h], ad + 2 * k, bd + 2 * k, k > 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc[0]);
+        wgmma_fence_acc(acc[1]);
+        if (lane == 0) mbar_arrive(&a_empty[slot]);
         float* drow = s_d + (j & 3) * D_SLOT;
 #pragma unroll
-        for (int k = 0; k < 27; ++k) drow[k * D_PITCH + t] = __uint_as_float(v[k]);
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int col = 64 * h + 16 * warp + (lane >> 2) + 8 * half;
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int k = 8 * q + cq + e;
+                if (k < 27) drow[k * D_PITCH + col] = acc[h][4 * q + 2 * half + e];
+              }
+          }
         named_bar_sync(1, 128);
         if (j >= 2) {
           const int yo = ys + j - 2;
@@ -411,9 +355,6 @@ conv0_bwd_kernel(const __grid_constant__ CUtensorMap tm_g0, const bf16* __restri
       named_bar_sync(1, 128);  // the next item restarts the D ring at slot 0
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<BW_RING * 32>(tmem_base);
 }
 
 __global__ void pack_w0_bwd_q_kernel(const float* __restrict__ w0, bf16* __restrict__ out) {
@@ -438,7 +379,7 @@ int launch_conv0_fwd(const float* img, const bf16* w0_packed, const float* bias,
   CUtensorMap tm;
   STB_TRY(make_tmap_bf16_3d(&tm, out, 64, W, H, 128ull, (uint64_t)W * 128ull, 64, W < C0_PX ? W : C0_PX, 1));
   const int n_items = ((H + C0_ROWS - 1) / C0_ROWS) * ((W + C0_PX - 1) / C0_PX);
-  const int grid = n_items < 2 * num_sms() ? n_items : 2 * num_sms();  // two CTAs per SM (92 KiB smem, 128 TMEM columns each)
+  const int grid = n_items < 2 * num_sms() ? n_items : 2 * num_sms();  // two CTAs per SM (92 KiB smem each)
   conv0_fwd_kernel<<<grid, C0_THREADS, C0_SMEM, s>>>(img, w0_packed, bias, tm, H, W);
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;

@@ -1,21 +1,23 @@
-// tcgen05 / TMEM / TMA implicit-GEMM for the VGG-19 3x3 convolutions (forward and dgrad) and the per-tap
-// feature-gradient GEMM, on NHWC bf16 activations with fp32 accumulation in tensor memory.
+// wgmma / TMA implicit-GEMM for the VGG-19 3x3 convolutions (forward and dgrad) and the per-tap feature-gradient
+// GEMM, on NHWC bf16 activations with fp32 accumulation in registers.
 //
-// Replaces, on the reference's hot path (ST = /root/reference/style_transfer/style_transfer.py):
+// Replaces, on the reference's hot path (ST = style_transfer/style_transfer.py of the reference):
 //   * ST:86-89  `self.model[i](input)` for the twelve 3x3/zero-pad convs + ReLU(inplace)  (torchvision vgg.py:73-87)
 //   * ST:475    `loss.backward()` through those convs (cuDNN/oneDNN backward-data; weights frozen at ST:49, so no
 //               wgrad), the ReLU `threshold_backward`, and the Gram/mean backward `dL/dF = F(G+G^T)/N + 1 gmu^T/N`
-//               of ST:163-168 which is folded in as extra K-blocks accumulating into the same TMEM tile.
+//               of ST:163-168 which is folded in as extra K-blocks accumulating into the same accumulators.
 //
-// Tiling: one CTA tile = MT horizontally adjacent sub-tiles of 16x8 output pixels (M = 128 TMEM lanes each) x BN
-// output channels (BN in {64,128,256} fp32 TMEM columns; MT = 2 for BN <= 128 so that every weight stage feeds two
-// sub-tiles), K = 9 taps x Cin.  Persistent CTAs (one per SM) walk tiles; three roles:
-//   warp 0      TMA producer: per 64-channel chunk it loads three "dx buffers" (18 rows x 8 px x 64 ch, SW128,
+// Tiling: one CTA tile = MT horizontally adjacent sub-tiles of 16x8 output pixels (M = 128 each) x BN output channels
+// (BN in {64,128,256}; MT = 2 for BN <= 128 so that every weight stage feeds two sub-tiles), K = 9 taps x Cin.
+// Persistent CTAs (one per SM) walk tiles; roles:
+//   warp 8      TMA producer (the only active warp of warpgroup 2, which gives its registers to the consumers):
+//               per 64-channel chunk it loads three "dx buffers" (18 rows x 8 px x 64 ch, SW128,
 //               zero-filled out of bounds = the conv's zero padding); the three dy taps are 1 KiB-aligned row
 //               shifts inside a dx buffer, so each activation byte is fetched 3.4x instead of 9x from L2.
 //               Weights stream tap by tap through a second ring.
-//   warp 1      single-thread tcgen05.mma issuer (kind::f16, bf16 x bf16 -> fp32), double-buffered accumulators.
-//   warps 2-5   epilogue: tcgen05.ld -> bias/ReLU or mask/content -> bf16 -> swizzled smem -> TMA store.
+//   warps 0-7   two consumer warpgroups: warpgroup g owns pixel rows 8g .. 8g+7 of every sub-tile (M = 64), issues
+//               its wgmma (bf16 x bf16 -> fp32 registers, one MMA group in flight while the next is issued), then
+//               runs the epilogue: bias/ReLU or mask/content -> bf16 -> swizzled smem -> TMA store (+ fused pool).
 #include <cstdlib>
 
 #include "kernels.h"
@@ -25,39 +27,34 @@ namespace stb {
 
 namespace {
 
-constexpr int TILE_H = 16, TILE_W = 8;           // output pixels per sub-tile = 128 = UMMA M
+constexpr int TILE_H = 16, TILE_W = 8;           // output pixels per sub-tile = 128 = two wgmma M blocks
 constexpr int A_ROWS = TILE_H + 2;               // dx buffer rows (halo above/below)
-constexpr int STG_BYTES = TILE_H * 1024;         // 128 pixels x 64 ch bf16 staging for the TMA store
-constexpr int PSTG_BYTES = (TILE_H / 2) * (TILE_W / 2) * 128;
-constexpr int NUM_EPI_THREADS = 128;   // one epilogue group = 4 warps = the 128 TMEM lanes
+constexpr int HALF_H = TILE_H / 2;               // pixel rows of one consumer warpgroup
+constexpr int STG_BYTES = HALF_H * 1024;         // 64 pixels x 64 ch bf16 staging for the TMA store
+constexpr int PSTG_BYTES = (HALF_H / 2) * (TILE_W / 2) * 128;
+constexpr int NUM_CONSUMERS = 256;               // two warpgroups
+constexpr int NUM_THREADS = NUM_CONSUMERS + 128; // + the producer warpgroup
 
 // MT = horizontally adjacent 16x8 sub-tiles per CTA tile that share every weight stage (halves the L2->smem
-// weight traffic per MMA for the narrow-N layers, which are L2-bandwidth bound otherwise).
+// weight traffic per MMA for the narrow-N layers).
 template <int BN>
 struct Cfg {
   static constexpr int MT = BN == 256 ? 1 : 2;
-  // Epilogue groups.  With N = 64 a sub-tile's MMAs last ~1150 cycles (36 x 32), less than its epilogue (TMEM load,
-  // mask / pool reads, bf16 pack, swizzled staging, TMA store): the C = 64 layers were epilogue-paced (37-50 % tensor
-  // pipe in round 1).  They get TWO groups of four warps, one per sub-tile, each with its own staging buffer.
-  static constexpr int EG = BN == 64 ? 2 : 1;
-  static constexpr int NUM_THREADS = 64 + EG * NUM_EPI_THREADS;
   static constexpr int NA = 3;
-  static constexpr int NB = BN == 64 ? 8 : 4;
+  static constexpr int NB = 4;
   static constexpr int A_PITCH = MT * 1024;                 // bytes per row of 8*MT pixels
   static constexpr int A_STAGE_BYTES = A_ROWS * A_PITCH;    // dx buffer: 18 rows x 8*MT px x 64 ch
   static constexpr int A2_BYTES = TILE_H * A_PITCH;         // centre box for the 1x1 source
   static constexpr int B_STAGE_BYTES = BN * 128;
-  static constexpr int TMEM_COLS = 2 * MT * BN;
   static constexpr int OFF_A = 0;
   static constexpr int OFF_B = OFF_A + NA * A_STAGE_BYTES;
-  static_assert(TMEM_COLS <= 512, "TMEM budget");
-  static constexpr int OFF_STG = OFF_B + NB * B_STAGE_BYTES;
-  static constexpr int OFF_PSTG = OFF_STG + 2 * STG_BYTES;  // 2 x 4 KiB: pooled 8x4-pixel tile of the fused 2x2 pool
-  static constexpr int OFF_BIAS = OFF_PSTG + 2 * PSTG_BYTES;
+  static constexpr int OFF_STG = OFF_B + NB * B_STAGE_BYTES;   // 2 warpgroups x 2 store staging buffers
+  static constexpr int OFF_PSTG = OFF_STG + 4 * STG_BYTES;     // 2 x 2 x 2 KiB: pooled 4x4-pixel tile of the fused pool
+  static constexpr int OFF_BIAS = OFF_PSTG + 4 * PSTG_BYTES;
   static constexpr int OFF_BAR = OFF_BIAS + 512 * 4;
-  static constexpr int NUM_BARS = 2 * NA + 2 * NB + 4;
-  static constexpr int OFF_TMEMPTR = OFF_BAR + NUM_BARS * 8;
-  static constexpr int SMEM_BYTES = OFF_TMEMPTR + 16 + 1024;  // + slack for manual 1 KiB alignment
+  static constexpr int NUM_BARS = 2 * NA + 2 * NB;
+  static constexpr int SMEM_BYTES = OFF_BAR + NUM_BARS * 8 + 1024;  // + slack for manual 1 KiB alignment
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 };
 
 struct KParams {
@@ -70,12 +67,11 @@ struct KParams {
   float cscale;
   int row_lo, row_hi;
   int pooling;  // MODE 0: -1 = none, else STB_POOL_*: also emit the 2x2-pooled output (tmPool)
-  int mma_interleave;  // issue order of the MT sub-tiles' MMAs (see the issuer loop)
-  int y_origin;        // first output row of the tile grid (row window of a band that computes its own rows only)
+  int y_origin; // first output row of the tile grid (row window of a band that computes its own rows only)
 };
 
 template <int BN, int MODE>
-__global__ void __launch_bounds__(Cfg<BN>::NUM_THREADS, 1)
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                   const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmPool,
@@ -89,9 +85,6 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* a_empty = a_full + C::NA;
   uint64_t* b_full = a_empty + C::NA;
   uint64_t* b_empty = b_full + C::NB;
-  uint64_t* t_full = b_empty + C::NB;   // [2]
-  uint64_t* t_empty = t_full + 2;       // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + C::OFF_TMEMPTR);
   float* s_bias = reinterpret_cast<float*>(smem + C::OFF_BIAS);
 
   const int warp = threadIdx.x >> 5;
@@ -100,34 +93,31 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int n_chunks2 = p.C2 >> 6;
 
   // ---- one-time setup
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmA2);
     tma_prefetch_desc(&tmB2);
     tma_prefetch_desc(&tmOut);
     tma_prefetch_desc(&tmPool);
-    for (int i = 0; i < C::NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < C::NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], 4 * C::EG); }
+    // empty barriers: one arrival per consumer warp once its wgmma reads of the stage are complete
+    for (int i = 0; i < C::NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
+    for (int i = 0; i < C::NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   // Programmatic dependent launch (see launch_cfg): everything above touched no global data and may have run while
   // the previous kernel of the iteration was still draining; its outputs (activations, and in MODE 1 the bias = gmu
   // produced by the W2 chain) are read only from here on.
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  for (int i = threadIdx.x; i < p.Cout && i < 512; i += C::NUM_THREADS) s_bias[i] = p.bias ? p.bias[i] : 0.f;
+  for (int i = threadIdx.x; i < p.Cout && i < 512; i += NUM_THREADS) s_bias[i] = p.bias ? p.bias[i] : 0.f;
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // =============================================================== TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
       int sa = 0, sb = 0;
       uint32_t pa = 0, pb = 0;  // ring phases
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -162,56 +152,57 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer
-    // The whole warp walks the (warp-uniform) schedule and waits on the barriers; one elected lane issues the
-    // tcgen05.mma / commit instructions.  For N = 64 an MMA lasts only 32 cycles, so the issue path is kept short:
-    // loop-invariant descriptor high words, low words advanced by +2 per K step.
-    constexpr uint32_t idesc = umma_idesc_bf16(128, BN, 0, 0);
-    constexpr uint32_t a_hi = umma_desc_hi_sw128(C::A_PITCH);
-    constexpr uint32_t b_hi = umma_desc_hi_sw128(1024);
-    const uint32_t a_base0 = smem_u32(smem + C::OFF_A);
+  } else {
+    // =============================================================== consumers: MMA + epilogue
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;                      // pixel rows 8 wg .. 8 wg + 7 of every sub-tile
+    const int wq = warp & 3;
+    const int et = threadIdx.x & 127;              // thread inside the warpgroup
+    const uint32_t bar0 = 1 + 3 * wg;              // named barriers of this warpgroup
+    const uint32_t a_base0 = smem_u32(smem + C::OFF_A) + wg * HALF_H * C::A_PITCH;
     const uint32_t b_base0 = smem_u32(smem + C::OFF_B);
-    const bool leader = elect_one();
-    int sa = 0, sb = 0, acc = 0;
-    uint32_t pa = 0, pb = 0, pacc = 0;
+    int sa = 0, sb = 0;
+    uint32_t pa = 0, pb = 0;
+    int stg = 0;
+    float acc[C::MT][BN / 2];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      mbar_wait(&t_empty[acc], pacc ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * (C::MT * BN);
-      uint32_t accum = 0;  // 0 only for the first weight stage of the tile (per-sub-tile accumulators)
+      const int tn = tile % p.n_tiles_n;
+      const int t2 = tile / p.n_tiles_n;
+      const int tx = t2 % p.tiles_x, ty = t2 / p.tiles_x;
+      const int y0 = p.y_origin + ty * TILE_H + wg * HALF_H, n0 = tn * BN;
+      // Stages are released one MMA group late: after issuing group g, wait until only g is in flight, then hand
+      // the stages of group g-1 back to the producer.
+      int rel_b = -1, rel_a = -1;
+      uint32_t accum = 0;  // 0 only for the first weight stage of the tile
+      auto release = [&](int keep) {
+        if (keep) wgmma_wait<1>(); else wgmma_wait<0>();
+        if (lane == 0) {
+          if (rel_b >= 0) mbar_arrive(&b_empty[rel_b]);
+          if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+        }
+      };
+      auto mma_stage = [&](uint32_t a_stage, int b_slot, int a_release) {
+        const uint64_t bd = gmma_desc_k(b_base0 + b_slot * C::B_STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int m = 0; m < C::MT; ++m) {
+          const uint64_t ad = gmma_desc_k(a_stage + m * 1024, C::A_PITCH);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_bf16<0, 0>(acc[m], ad + 2 * k, bd + 2 * k, accum | (k > 0));
+        }
+        wgmma_commit();
+        release(1);
+        rel_b = b_slot;
+        rel_a = a_release;
+        accum = 1;
+      };
       for (int c = 0; c < n_chunks; ++c) {
         for (int dx = 0; dx < 3; ++dx) {
           mbar_wait(&a_full[sa], pa);
           const uint32_t a_stage = a_base0 + sa * C::A_STAGE_BYTES;
           for (int dy = 0; dy < 3; ++dy) {
             mbar_wait(&b_full[sb], pb);
-            tc_fence_after();
-            if (leader) {
-              const uint32_t b_lo = umma_desc_lo(b_base0 + sb * C::B_STAGE_BYTES);
-              // experiment (STB_MMA_ORDER=1): k outer, sub-tile inner, so that two consecutive MMAs never accumulate into
-              // the same TMEM tile.  Measured slower than the default order below.
-              if (p.mma_interleave) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-#pragma unroll
-                  for (int m = 0; m < C::MT; ++m)
-                    umma_bf16_split(tmem_d + m * BN, umma_desc_lo(a_stage + dy * C::A_PITCH + m * 1024) + 2 * k, a_hi,
-                                    b_lo + 2 * k, b_hi, idesc, accum | (k > 0));
-              } else {
-#pragma unroll
-                for (int m = 0; m < C::MT; ++m) {
-                  const uint32_t a_lo = umma_desc_lo(a_stage + dy * C::A_PITCH + m * 1024);
-#pragma unroll
-                  for (int k = 0; k < 4; ++k)
-                    umma_bf16_split(tmem_d + m * BN, a_lo + 2 * k, a_hi, b_lo + 2 * k, b_hi, idesc, accum | (k > 0));
-                }
-              }
-              umma_commit(&b_empty[sb]);
-              if (dy == 2) umma_commit(&a_empty[sa]);
-            }
-            __syncwarp();
-            accum = 1;
+            mma_stage(a_stage + dy * C::A_PITCH, sb, dy == 2 ? sa : -1);
             if (++sb == C::NB) { sb = 0; pb ^= 1; }
           }
           if (++sa == C::NA) { sa = 0; pa ^= 1; }
@@ -220,145 +211,79 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       for (int c = 0; c < n_chunks2; ++c) {
         mbar_wait(&a_full[sa], pa);
         mbar_wait(&b_full[sb], pb);
-        tc_fence_after();
-        if (leader) {
-          constexpr uint32_t a2_hi = umma_desc_hi_sw128(C::A_PITCH);
-          const uint32_t b_lo = umma_desc_lo(b_base0 + sb * C::B_STAGE_BYTES);
-#pragma unroll
-          for (int m = 0; m < C::MT; ++m) {
-            const uint32_t a_lo = umma_desc_lo(a_base0 + sa * C::A_STAGE_BYTES + m * 1024);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_bf16_split(tmem_d + m * BN, a_lo + 2 * k, a2_hi, b_lo + 2 * k, b_hi, idesc, accum | (k > 0));
-          }
-          umma_commit(&b_empty[sb]);
-          umma_commit(&a_empty[sa]);
-        }
-        __syncwarp();
-        accum = 1;
+        mma_stage(a_base0 + sa * C::A_STAGE_BYTES, sb, sa);
         if (++sb == C::NB) { sb = 0; pb ^= 1; }
         if (++sa == C::NA) { sa = 0; pa ^= 1; }
       }
-      if (leader) umma_commit(&t_full[acc]);
-      __syncwarp();
-      if (++acc == 2) { acc = 0; pacc ^= 1; }
-    }
-  } else {
-    // =============================================================== epilogue (4 warps per group, TMEM lane group =
-    // warp % 4; EG groups split the sub-tiles of a CTA tile between them)
-    const int wq = warp & 3;
-    const int r = wq * 32 + lane;         // row of the tile = TMEM lane = pixel
-    const int grp = (threadIdx.x - 64) / NUM_EPI_THREADS;
-    const int et = (threadIdx.x - 64) % NUM_EPI_THREADS;      // 0..127 inside the group
-    const uint32_t bar0 = 1 + 3 * grp;    // named barriers of this group
-    int acc = 0;
-    uint32_t pacc = 0;
-    int stg = C::EG == 2 ? grp : 0;       // two groups: each owns one staging buffer
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int tn = tile % p.n_tiles_n;
-      const int t2 = tile / p.n_tiles_n;
-      const int tx = t2 % p.tiles_x, ty = t2 / p.tiles_x;
-      const int y0 = p.y_origin + ty * TILE_H, n0 = tn * BN;
-      mbar_wait(&t_full[acc], pacc);
-      tc_fence_after();
-#pragma unroll 1
-      for (int mj = (C::EG == 2 ? grp : 0); mj < C::MT * (BN / 64); mj += C::EG) {
-        const int m = mj / (BN / 64), j = mj % (BN / 64);
+      release(0);
+#pragma unroll
+      for (int m = 0; m < C::MT; ++m) wgmma_fence_acc(acc[m]);
+
+      // ---- epilogue: this warpgroup's 8 x 8 pixels of sub-tile m, 64 channels (j) at a time
+      const int rr = wq * 16 + (lane >> 2);        // pixel (row) of the first accumulator row held by this thread
+      const int cq = 2 * (lane & 3);               // first of the two columns held per 8-column group
+#pragma unroll
+      for (int m = 0; m < C::MT; ++m) {
         const int x0 = (tx * C::MT + m) * TILE_W;
-        const int py = y0 + (r >> 3), px = x0 + (r & 7);
-        const bool inb = (py < p.H) && (px < p.W);
-        const bool in_rows = (py >= p.row_lo) && (py < p.row_hi);
-        const size_t pix_off = (static_cast<size_t>(py) * p.W + px) * p.Cout + n0;
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16) + (acc * C::MT + m) * BN;
-        uint8_t* stage = smem + C::OFF_STG + stg * STG_BYTES;
-        // make sure the TMA store that last read this staging buffer is done, then let everyone write
-        if (et == 0) {
-          if (C::EG == 2) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // single buffer per group
-          else asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        }
-        named_bar_sync(bar0, NUM_EPI_THREADS);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t v[32];
-          tmem_ld_32x32(taddr + j * 64 + h * 32, v);
-          tmem_ld_wait();
-          const int cb = j * 64 + h * 32;  // column base inside the N tile
-          uint32_t packed[16];
-          if (MODE == 0) {
+        for (int j = 0; j < BN / 64; ++j) {
+          uint8_t* stage = smem + C::OFF_STG + (2 * wg + stg) * STG_BYTES;
+          // make sure the TMA store that last read this staging buffer is done, then let everyone write
+          if (et == 0) tma_store_wait_read<1>();
+          named_bar_sync(bar0, 128);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float a = __uint_as_float(v[2 * i]) + s_bias[n0 + cb + 2 * i];
-              float b = __uint_as_float(v[2 * i + 1]) + s_bias[n0 + cb + 2 * i + 1];
-              packed[i] = pack_bf16x2(fmaxf(a, 0.f), fmaxf(b, 0.f));
-            }
-          } else if (MODE == 2) {
+          for (int half = 0; half < 2; ++half) {
+            const int r = rr + 8 * half;
+            const int py = y0 + (r >> 3), px = x0 + (r & 7);
+            const bool inb = (py < p.H) && (px < p.W);
+            const bool in_rows = (py >= p.row_lo) && (py < p.row_hi);
+            const bool has_c = (p.ctarget != nullptr) && in_rows && inb;
+            const size_t pix_off = (static_cast<size_t>(py) * p.W + px) * p.Cout + n0 + j * 64 + cq;
 #pragma unroll
-            for (int i = 0; i < 16; ++i)
-              packed[i] = pack_bf16x2(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1]));
-          } else {
-            uint4 yv[4], tv[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              yv[q] = make_uint4(0, 0, 0, 0);
-              tv[q] = make_uint4(0, 0, 0, 0);
-            }
-            if (inb) {
-              const uint4* yp = reinterpret_cast<const uint4*>(p.mask_src + pix_off + cb);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) yv[q] = __ldg(yp + q);
-              if (p.ctarget != nullptr && in_rows) {
-                const uint4* tp = reinterpret_cast<const uint4*>(p.ctarget + pix_off + cb);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) tv[q] = __ldg(tp + q);
+            for (int q = 0; q < 8; ++q) {
+              const int cb = j * 64 + q * 8 + cq;    // column inside the N tile
+              float a = acc[m][(j * 8 + q) * 4 + 2 * half], b = acc[m][(j * 8 + q) * 4 + 2 * half + 1];
+              uint32_t packed;
+              if (MODE == 0) {
+                packed = pack_bf16x2(fmaxf(a + s_bias[n0 + cb], 0.f), fmaxf(b + s_bias[n0 + cb + 1], 0.f));
+              } else if (MODE == 2) {
+                packed = pack_bf16x2(a, b);
+              } else {
+                const uint32_t yw = inb ? __ldg(reinterpret_cast<const unsigned*>(p.mask_src + pix_off + q * 8)) : 0u;
+                const float ya = bf16lo(yw), yb = bf16hi(yw);
+                if (in_rows) {
+                  a += s_bias[n0 + cb];
+                  b += s_bias[n0 + cb + 1];
+                }
+                if (has_c) {
+                  const uint32_t tw = __ldg(reinterpret_cast<const unsigned*>(p.ctarget + pix_off + q * 8));
+                  a += p.cscale * (ya - bf16lo(tw));
+                  b += p.cscale * (yb - bf16hi(tw));
+                }
+                packed = pack_bf16x2(ya > 0.f ? a : 0.f, yb > 0.f ? b : 0.f);
               }
-            }
-            const uint32_t* yw = reinterpret_cast<const uint32_t*>(yv);
-            const uint32_t* tw = reinterpret_cast<const uint32_t*>(tv);
-            const bool has_c = (p.ctarget != nullptr) && in_rows;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float ya = bf16lo(yw[i]), yb = bf16hi(yw[i]);
-              float a = __uint_as_float(v[2 * i]);
-              float b = __uint_as_float(v[2 * i + 1]);
-              if (in_rows) {
-                a += s_bias[n0 + cb + 2 * i];
-                b += s_bias[n0 + cb + 2 * i + 1];
-              }
-              if (has_c) {
-                a += p.cscale * (ya - bf16lo(tw[i]));
-                b += p.cscale * (yb - bf16hi(tw[i]));
-              }
-              packed[i] = pack_bf16x2(ya > 0.f ? a : 0.f, yb > 0.f ? b : 0.f);
+              // swizzled (SW128) staging write: 16-byte chunk q of pixel r lives at chunk (q ^ (r & 7))
+              *reinterpret_cast<uint32_t*>(stage + r * 128 + ((q ^ (r & 7)) << 4) + cq * 2) = packed;
             }
           }
-          // swizzled (SW128) staging write: 16-byte chunk c16 of row r lives at chunk (c16 ^ (r & 7))
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int c16 = h * 4 + q;
-            uint4* dst = reinterpret_cast<uint4*>(stage + r * 128 + ((c16 ^ (r & 7)) << 4));
-            *dst = make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
+          fence_proxy_async_smem();
+          named_bar_sync(bar0 + 1, 128);
+          const bool pooled = (MODE == 0) && p.pooling >= 0;
+          if (et == 0) {
+            tma_store_3d(&tmOut, stage, n0 + j * 64, x0, y0);
+            if (!pooled) tma_store_commit();
           }
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(bar0 + 1, NUM_EPI_THREADS);
-        const bool pooled = (MODE == 0) && p.pooling >= 0;
-        if (et == 0) {
-          tma_store_3d(&tmOut, stage, n0 + j * 64, x0, y0);
-          if (!pooled) tma_store_commit();
-        }
-        if (MODE == 0 && pooled) {
-          // fused 2x2 / stride-2 pool (ST:21-22, 41-46) of the tile just staged: 8 x 4 pooled pixels x 8 chunks of
-          // 8 channels = 256 tasks; windows never straddle tiles (tile origin and size are even)
-          uint8_t* pst = smem + C::OFF_PSTG + stg * PSTG_BYTES;
-#pragma unroll
-          for (int task = et; task < 256; task += NUM_EPI_THREADS) {
-            const int pp = task >> 3, c16 = task & 7;
-            const int r0 = ((pp >> 2) * 2) * TILE_W + (pp & 3) * 2;  // top-left source pixel (row of the tile)
+          if (MODE == 0 && pooled) {
+            // fused 2x2 / stride-2 pool (ST:21-22, 41-46) of the 8x8 pixels just staged: 4 x 4 pooled pixels x 8
+            // chunks of 8 channels = 128 tasks; windows never straddle tiles (origin and size are even)
+            uint8_t* pst = smem + C::OFF_PSTG + (2 * wg + stg) * PSTG_BYTES;
+            const int pp = et >> 3, c16 = et & 7;
+            const int r0 = ((pp >> 2) * 2) * TILE_W + (pp & 3) * 2;  // top-left source pixel
             uint4 v[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
-              const int rr = r0 + (q >> 1) * TILE_W + (q & 1);
-              v[q] = *reinterpret_cast<const uint4*>(stage + rr * 128 + ((c16 ^ (rr & 7)) << 4));
+              const int rs = r0 + (q >> 1) * TILE_W + (q & 1);
+              v[q] = *reinterpret_cast<const uint4*>(stage + rs * 128 + ((c16 ^ (rs & 7)) << 4));
             }
             uint32_t o[4];
 #pragma unroll
@@ -384,29 +309,19 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               o[k] = pack_bf16x2(a, b);
             }
             *reinterpret_cast<uint4*>(pst + pp * 128 + ((c16 ^ (pp & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+            fence_proxy_async_smem();
+            named_bar_sync(bar0 + 2, 128);
+            if (et == 0) {
+              tma_store_3d(&tmPool, pst, n0 + j * 64, x0 >> 1, y0 >> 1);
+              tma_store_commit();
+            }
           }
-          fence_proxy_async_smem();
-          named_bar_sync(bar0 + 2, NUM_EPI_THREADS);
-          if (et == 0) {
-            tma_store_3d(&tmPool, pst, n0 + j * 64, x0 >> 1, y0 >> 1);
-            tma_store_commit();
-          }
+          stg ^= 1;
         }
-        if (C::EG == 1) stg ^= 1;
       }
-      // accumulator drained -> hand the TMEM buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&t_empty[acc]);
-      if (++acc == 2) { acc = 0; pacc ^= 1; }
     }
     if (et == 0) tma_store_wait_all0();
   }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<C::TMEM_COLS>(tmem_base);
 }
 
 template <int BN, int MODE>
@@ -421,7 +336,7 @@ int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap
   static const bool pdl = [] { const char* e = getenv("STB_PDL"); return !(e && e[0] == '0'); }();
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(C::NUM_THREADS);
+  cfg.blockDim = dim3(NUM_THREADS);
   cfg.dynamicSmemBytes = C::SMEM_BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute at[1];
@@ -458,18 +373,13 @@ int launch_pixel_gemm(const PixelGemmArgs& a, cudaStream_t stream) {
   kp.a2_row0 = a.a2_row0;
   kp.bias = a.bias; kp.mask_src = a.mask_src; kp.ctarget = a.ctarget; kp.cscale = a.cscale;
   kp.row_lo = a.row_lo; kp.row_hi = a.row_hi;
-  // default: sub-tile-major (four k-steps of one sub-tile back to back).  The k-major order (STB_MMA_ORDER=1) was tried
-  // against the hypothesis that dependent accumulations stall the pipe: under ncu it is 8-17 % SLOWER on the N <= 128
-  // launches (alternating A descriptors), see DESIGN.md section 4.1.
-  static const int mma_order = [] { const char* e = getenv("STB_MMA_ORDER"); return (e && e[0] == '1') ? 1 : 0; }();
-  kp.mma_interleave = mma_order;
   STB_CHECK(a.mode >= 0 && a.mode <= 2, STB_ERR_INVALID, "pixel_gemm: mode=%d", a.mode);
   if (a.mode == 1) STB_CHECK(a.mask_src != nullptr, STB_ERR_INVALID, "pixel_gemm: bwd needs mask_src");
 
   CUtensorMap tmA, tmB, tmA2, tmB2, tmOut, tmPool;
   const uint64_t W = a.W, H = a.H;
   // output first; unused maps alias it so that every descriptor handed to the kernel is valid
-  STB_TRY(make_tmap_bf16_3d(&tmOut, a.out, a.Cout, W, H, a.Cout * 2ull, W * a.Cout * 2ull, 64, TILE_W, TILE_H));
+  STB_TRY(make_tmap_bf16_3d(&tmOut, a.out, a.Cout, W, H, a.Cout * 2ull, W * a.Cout * 2ull, 64, TILE_W, HALF_H));
   tmA = tmB = tmA2 = tmB2 = tmPool = tmOut;
   kp.pooling = -1;
   if (a.pool_out != nullptr) {
@@ -477,7 +387,7 @@ int launch_pixel_gemm(const PixelGemmArgs& a, cudaStream_t stream) {
               "pixel_gemm: fused pool needs mode 0 and a valid pooling");
     kp.pooling = a.pooling;
     STB_TRY(make_tmap_bf16_3d(&tmPool, a.pool_out, a.Cout, W / 2, H / 2, a.Cout * 2ull, (W / 2) * a.Cout * 2ull, 64,
-                              TILE_W / 2, TILE_H / 2));
+                              TILE_W / 2, HALF_H / 2));
   }
   if (a.Cin > 0) {
     STB_TRY(make_tmap_bf16_3d(&tmA, a.A, a.Cin, W, H, a.Cin * 2ull, W * a.Cin * 2ull, 64, tile_w, A_ROWS));

@@ -1,23 +1,20 @@
-// Second raw moment and channel sums of a pixel-major (NHWC bf16) activation on tcgen05:
+// Second raw moment and channel sums of a pixel-major (NHWC bf16) activation on wgmma:
 //     S_raw[i][j] = sum_p F[p][i] * F[p][j]        sums[i] = sum_p F[p][i]
 // i.e. the un-normalised `einsum('...chw,...dhw->...cd')` and `mean([-2,-1])` of StyleLossW2.get_target
-// (/root/reference/style_transfer/style_transfer.py:163-168).  K is the pixel axis (up to 4.2 M), so the GEMM is
-// split-K: CTA (tile, split) accumulates a 128 x BN fp32 tile in TMEM over its pixel range and writes a partial;
-// gram_reduce sums the partials in a fixed order (deterministic).
+// (style_transfer/style_transfer.py:163-168 of the reference).  K is the pixel axis (up to 4.2 M), so the GEMM is
+// split-K: CTA (tile, split) accumulates a 128 x BN fp32 tile over its pixel range and writes a partial; gram_reduce
+// sums the partials in a fixed order (deterministic).
 //
 // Accuracy: the tensor core adds into its fp32 accumulator with TRUNCATION, and here every product is >= 0 (post-ReLU
-// features), so a chain of n k-steps loses ~n * 2^-24.5 of the sum -- systematically.  At 2048^2 the relu1_1 chain is
-// 1771 steps per CTA (-8e-5), which the covariance (S/N - mu mu^T) and the W2 cancellation amplify ~200x into a
-// -1 % error of that style term (measured: -0.27 % at 1024^2).  For C <= 128 the accumulator is therefore double
-// buffered in TMEM and DRAINED every 32 k-steps into fp32 registers of the epilogue warps (round-to-nearest adds),
-// which overlaps with the next chunk's MMAs and costs nothing on these HBM-bound layers.  C >= 256 (no TMEM room for
-// a second 256-column set) ran on one set in round 1; the reference-pinned checks at 1024^2 ... 4096^2 showed its style
-// terms drifting with the pixel count (relu3_1: 0.7e-3 at 512^2 -> 2.0e-3 at 4096^2), so C >= 256 now runs as 128 x 128
-// tiles of the UPPER triangle with the same drain (GCfg<128, true>: separate A atoms, 64-pixel stages); the lower
-// triangle is mirrored by the reduction.
+// features), so a long chain of k-steps loses ~n * 2^-24.5 of the sum -- systematically, and the covariance
+// (S/N - mu mu^T) and the W2 cancellation amplify that ~200x.  The MMA accumulator is therefore restarted every 32
+// k-steps and DRAINED into a second set of fp32 registers (round-to-nearest adds).  C >= 256 runs as 128 x 128 tiles
+// of the UPPER triangle (GCfg<128, true>: separate A atoms, 64-pixel stages); the lower triangle is mirrored by the
+// reduction.
 //
 // Both operands are the SAME pixel-major smem tiles read "MN-major" (channel contiguous, SW128): no transpose is
 // ever materialised.  Channel sums ride along as one extra N=16 MMA per k-step against a constant tile of ones.
+// Roles: two consumer warpgroups (rows i0 .. i0+63 and i0+64 .. i0+127 of the tile), one TMA producer warp.
 #include <cstdlib>
 
 #include "kernels.h"
@@ -28,7 +25,7 @@ namespace stb {
 namespace {
 
 constexpr int G_STAGES = 4;
-constexpr int G_THREADS = 64 + 128;
+constexpr int G_THREADS = 256 + 32;
 constexpr int PK_MAX = 256;
 
 // PK = pixels per pipeline stage.  The narrow layers are pure HBM streams (C = 64: 8 KiB per 64 pixels), so they get
@@ -40,17 +37,13 @@ struct GCfg {
   static constexpr int PK = BN == 64 ? 256 : (BN == 128 ? (SEP ? 64 : 128) : 64);
   static constexpr int ATOM_BYTES = PK * 128;   // 64 channels x PK pixels, bf16
   static constexpr int B_ATOMS = BN / 64;
-  static constexpr int A_ATOMS = (BN == 256 || SEP) ? 2 : 0;  // C <= 128: the A block is always contained in the B block
+  static constexpr int A_ATOMS = SEP ? 2 : 0;   // C <= 128: the A block is always contained in the B block
   static constexpr int STAGE_BYTES = (B_ATOMS + A_ATOMS) * ATOM_BYTES;
-  // + one atom of slack: with C = 64 the (ignored) upper 64 accumulator rows read one atom past the stage
+  // + one atom of slack: with C = 64 the (discarded) rows 64..127 of the second warpgroup read one atom past the stage
   static constexpr int OFF_ONES = G_STAGES * STAGE_BYTES + ATOM_BYTES;
   static constexpr int OFF_BAR = OFF_ONES + 2048;
-  static constexpr int OFF_TMEMPTR = OFF_BAR + (2 * G_STAGES + 4) * 8;
-  static constexpr int SMEM_BYTES = OFF_TMEMPTR + 16 + 1024;
-  static constexpr bool DRAIN = BN <= 128;
-  static constexpr int SET_COLS = BN + 32;                    // BN Gram columns + 16 channel-sum columns (+ pad)
-  static constexpr int TMEM_COLS = BN == 256 ? 512 : (BN == 128 ? 512 : 256);
-  static constexpr int CHUNK_STAGES = DRAIN ? 32 / (PK / 16) : (1 << 30);  // stages per 32-k-step chunk
+  static constexpr int SMEM_BYTES = OFF_BAR + 2 * G_STAGES * 8 + 1024;
+  static constexpr int CHUNK_STAGES = 32 / (PK / 16);   // stages per 32-k-step chunk
 };
 
 struct GParams {
@@ -71,9 +64,6 @@ gram_kernel(const __grid_constant__ CUtensorMap tmF, const GParams p) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
   uint64_t* empty = full + G_STAGES;
-  uint64_t* t_full = empty + G_STAGES;  // [2]
-  uint64_t* t_empty = t_full + 2;       // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + C::OFF_TMEMPTR);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int ti = blockIdx.x / p.n_tj, tj = blockIdx.x % p.n_tj;
@@ -96,20 +86,16 @@ gram_kernel(const __grid_constant__ CUtensorMap tmF, const GParams p) {
   // constant ones tile (bf16 1.0 = 0x3F80)
   for (int i = threadIdx.x; i < 2048 / 4; i += G_THREADS)
     reinterpret_cast<uint32_t*>(smem + C::OFF_ONES)[i] = 0x3F803F80u;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmF);
-    for (int i = 0; i < G_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], 4); }
+    // empty: one arrival per consumer warp once its wgmma reads of the stage are complete
+    for (int i = 0; i < G_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<C::TMEM_COLS>(tmem_ptr);
   fence_proxy_async_smem();  // ones tile is read by the tensor core (async proxy)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       const uint32_t tx_bytes = (C::B_ATOMS + (contained ? 0 : C::A_ATOMS)) * ATOM_BYTES;
       int s = 0;
@@ -127,121 +113,73 @@ gram_kernel(const __grid_constant__ CUtensorMap tmF, const GParams p) {
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // whole warp walks the k loop, one elected lane issues (short issue path: split descriptors, see conv_tc.cu)
-    constexpr uint32_t idesc_main = umma_idesc_bf16(128, BN, 1, 1);
-    constexpr uint32_t idesc_sum = umma_idesc_bf16(128, 16, 1, 1);
-    constexpr uint32_t hi_mn = umma_desc_hi_sw128(1024);  // MN-major: SBO = stride between 8-pixel groups
-    const uint32_t ones_lo = umma_desc_lo(smem_u32(smem + C::OFF_ONES), 1024);
-    const bool leader = elect_one();
+  } else {
+    // ---- consumer warpgroup wg: Gram rows i0 + 64 wg .. i0 + 64 wg + 63 (discarded beyond m_valid).  The MMAs are
+    // issued unconditionally (channel sums included, kept on diagonal tiles only): a wgmma under a branch the compiler
+    // cannot prove uniform is serialised.
+    const int wg = warp >> 2, wq = warp & 3;
+    const bool diag = tj == ti;
+    const uint64_t ones = gmma_desc_k(smem_u32(smem + C::OFF_ONES));   // K-major, every element 1
+    float acc[BN / 2], tot[BN / 2], sacc[8], stot[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
     int s = 0;
-    uint32_t ph = 0, accum = 0;
-    for (int k = 0; k < n_k; ++k) {
-      const int chunk = k / C::CHUNK_STAGES, set = chunk & 1;
-      const bool chunk_first = (k % C::CHUNK_STAGES) == 0, chunk_last = ((k + 1) % C::CHUNK_STAGES) == 0 || k == n_k - 1;
-      if (chunk_first) {
-        if (C::DRAIN) mbar_wait(&t_empty[set], ((chunk >> 1) & 1) ^ 1);  // the epilogue has drained this set
-        accum = 0;
-      }
-      const uint32_t tmem_d = tmem_base + set * C::SET_COLS;
-      mbar_wait(&full[s], ph);
-      tc_fence_after();
-      if (leader) {
+    uint32_t ph = 0;
+    for (int k = 0; k < n_k;) {
+      // one chunk of (at most) 32 k-steps into a fresh accumulator; stage k-1 is released once only stage k's MMA
+      // group is still in flight
+      int prev = -1;
+      for (int kc = 0; kc < C::CHUNK_STAGES && k < n_k; ++kc, ++k) {
+        mbar_wait(&full[s], ph);
         const uint32_t b_addr = smem_u32(smem + s * C::STAGE_BYTES);
-        const uint32_t a_addr = contained ? b_addr + ((i0 - j0) >> 6) * ATOM_BYTES : b_addr + C::B_ATOMS * ATOM_BYTES;
-        // MN-major SW128: LBO = stride between 64-channel atoms
-        const uint32_t a_lo = umma_desc_lo(a_addr, ATOM_BYTES), b_lo = umma_desc_lo(b_addr, ATOM_BYTES);
+        const uint32_t a_addr =
+            (contained ? b_addr + ((i0 - j0) >> 6) * ATOM_BYTES : b_addr + C::B_ATOMS * ATOM_BYTES) + wg * ATOM_BYTES;
+        // MN-major SW128: LBO = stride between 64-channel atoms, SBO = 8 pixels; a 16-pixel K step is +2048 bytes
+        const uint64_t ad = gmma_desc(a_addr, ATOM_BYTES, 1024), bd = gmma_desc(b_addr, ATOM_BYTES, 1024);
+        wgmma_fence();
 #pragma unroll
         for (int ks = 0; ks < PK / 16; ++ks) {
-          umma_bf16_split(tmem_d, a_lo + ks * 128, hi_mn, b_lo + ks * 128, hi_mn, idesc_main, accum | (ks > 0));
-          if (tj == ti)
-            umma_bf16_split(tmem_d + BN, a_lo + ks * 128, hi_mn, ones_lo, hi_mn, idesc_sum, accum | (ks > 0));
+          const uint32_t sc = kc > 0 || ks > 0;
+          wgmma_bf16<1, 1>(acc, ad + ks * 128, bd + ks * 128, sc);
+          wgmma_bf16<1, 0>(sacc, ad + ks * 128, ones, sc);
         }
-        umma_commit(&empty[s]);
-        if (chunk_last) umma_commit(&t_full[set]);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == G_STAGES) { s = 0; ph ^= 1; }
       }
-      __syncwarp();
-      accum = 1;
-      if (++s == G_STAGES) { s = 0; ph ^= 1; }
+      wgmma_wait<0>();
+      if (lane == 0) mbar_arrive(&empty[prev]);
+      wgmma_fence_acc(acc);
+      wgmma_fence_acc(sacc);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) tot[i] += acc[i];
+      stot[0] += sacc[0];
+      stot[1] += sacc[2];
     }
-  } else {
-    const int wq = warp & 3;
-    const int r = wq * 32 + lane;
-    const bool valid = r < m_valid;
-    float* dst = p.partials + ((size_t)split * p.C + (i0 + r)) * p.C + j0;
-    const int n_chunks = (n_k + C::CHUNK_STAGES - 1) / C::CHUNK_STAGES;
-    if constexpr (C::DRAIN) {
-      // drain every finished 32-k-step chunk into registers (fp32, round to nearest); the MMAs of the next chunk run
-      // into the other TMEM set meanwhile
-      float acc[BN];
-      float acc_sum = 0.f;
+    if (n_k > 0) {
+      const int cq = 2 * (lane & 3);
 #pragma unroll
-      for (int i = 0; i < BN; ++i) acc[i] = 0.f;
-      for (int c = 0; c < n_chunks; ++c) {
-        const int set = c & 1;
-        mbar_wait(&t_full[set], (c >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + set * C::SET_COLS + (static_cast<uint32_t>(wq * 32) << 16);
+      for (int half = 0; half < 2; ++half) {
+        const int r = 64 * wg + 16 * wq + (lane >> 2) + 8 * half;
+        if (r < m_valid) {
+          float* dst = p.partials + ((size_t)split * p.C + (i0 + r)) * p.C + j0 + cq;
 #pragma unroll
-        for (int cb = 0; cb < BN; cb += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(taddr + cb, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc[cb + i] += __uint_as_float(v[i]);
+          for (int q = 0; q < BN / 8; ++q)
+            *reinterpret_cast<float2*>(dst + 8 * q) = make_float2(tot[4 * q + 2 * half], tot[4 * q + 2 * half + 1]);
+          if (diag && cq == 0) p.sum_partials[(size_t)split * p.C + i0 + r] = stot[half];
         }
-        if (tj == ti) {
-          uint32_t v[4];
-          tmem_ld_32x32_x4(taddr + BN, v);
-          tmem_ld_wait();
-          acc_sum += __uint_as_float(v[0]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&t_empty[set]);
-      }
-      if (valid && n_k > 0) {
-#pragma unroll
-        for (int q = 0; q < BN / 4; ++q)
-          *reinterpret_cast<float4*>(dst + 4 * q) = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
-        if (tj == ti) p.sum_partials[(size_t)split * p.C + i0 + r] = acc_sum;
-      }
-    } else {
-      if (n_chunks > 0) mbar_wait(&t_full[0], 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16);
-#pragma unroll 1
-      for (int cb = 0; cb < BN; cb += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(taddr + cb, v);
-        tmem_ld_wait();
-        if (valid && n_k > 0) {
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(dst + cb + 4 * q) =
-                make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                            __uint_as_float(v[4 * q + 3]));
-        }
-      }
-      if (tj == ti) {
-        uint32_t v[32];
-        tmem_ld_32x32(taddr + BN, v);
-        tmem_ld_wait();
-        if (valid && n_k > 0) p.sum_partials[(size_t)split * p.C + i0 + r] = __uint_as_float(v[0]);
       }
     }
-    tc_fence_before();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<C::TMEM_COLS>(tmem_base);
 }
 
 // sum partials in a fixed order: out[i] = sum_s part[s][i]; deterministic run to run.  One launch covers the Gram
 // partials (n0 elements) and the channel-sum partials (n1 elements, element index continues after n0).  A block owns
 // 64 elements; its 256 threads are 4 split-lanes x 64 elements: lane g adds the splits s = g, g+4, ... (4 interleaved
 // accumulators for memory-level parallelism), then the four lane sums are combined in order through shared memory.
-// (With one thread per element the C = 64 layer -- 148 splits, 4160 elements -- ran on 17 CTAs and took 40 us.)
+// (With one thread per element the C = 64 layer -- one split per SM, 4160 elements -- ran on 17 CTAs.)
 // mirror_c > 0: part0 is a [mirror_c][mirror_c] matrix of which only the 128 x 128 tiles of the upper triangle were
 // written; elements of the lower triangle read the transposed position (the Gram matrix is symmetric).
 __global__ void __launch_bounds__(256)
@@ -296,8 +234,7 @@ int preload_gram_kernels() {
   return STB_OK;
 }
 
-// C <= 128: one tile row, BN = C.  C >= 256: 128 x 128 tiles of the upper triangle (drained accumulators, see the
-// header), 64-pixel stages.
+// C <= 128: one tile row, BN = C.  C >= 256: 128 x 128 tiles of the upper triangle, 64-pixel stages.
 static int gram_bn(int C) { return C >= 128 ? 128 : C; }
 static bool gram_sep(int C) { return C >= 256; }
 static int gram_pk(int C) { return C == 64 ? 256 : (C == 128 ? 128 : 64); }

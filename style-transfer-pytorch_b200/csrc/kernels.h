@@ -11,7 +11,7 @@ namespace stb {
 
 typedef __nv_bfloat16 bf16;
 
-// ---------------------------------------------------------------- tcgen05 implicit-GEMM "pixel GEMM"
+// ---------------------------------------------------------------- wgmma implicit-GEMM "pixel GEMM"
 // out[p][n] = epilogue( sum_{tap,k} A[p + off(tap)][k] * B[tap][n][k]  +  sum_k A2[p][k] * B2[n][k] )
 //   fwd  (mode 0): + bias[n], ReLU                       (VGG conv 3x3 + bias + ReLU; ST:86-89 -> torchvision vgg.py)
 //   bwd  (mode 1): + bias[n] (rows in [row_lo,row_hi)), + cscale*(y - ctarget), * (y > 0)
@@ -53,7 +53,7 @@ struct AdamScalars {  // torch/optim/adam.py:413-546 scalars, evaluated on the h
 int launch_tv(const float* img, int H, int W, int row0, int rows, int H_norm, float tv_weight, float* gtv,
               float* tv_partials, int* n_partials, cudaStream_t s);
 int pack_weights_conv0_fwd(const float* w0, bf16* out, cudaStream_t s);
-// conv0 forward on tcgen05 with the im2col rows built in shared memory (conv0_tc.cu); out: bf16 NHWC [H][W][64]
+// conv0 forward on wgmma with the im2col rows built in shared memory (conv0_tc.cu); out: bf16 NHWC [H][W][64]
 int launch_conv0_fwd(const float* img, const bf16* w0_packed, const float* bias, bf16* out, int H, int W,
                      cudaStream_t s);
 // g0: masked gradient w.r.t. conv0's pre-activation, bf16 NHWC [H][W][64].  interior_done: the interior pixels were
@@ -62,7 +62,7 @@ int launch_conv0_fwd(const float* img, const bf16* w0_packed, const float* bias,
 int launch_conv0_bwd_adam(const bf16* g0, bool interior_done, const float* w0, const float* gtv, float* img,
                           float* exp_avg, float* exp_avg_sq, float* ema, float* grad_out, int H, int W,
                           const AdamScalars* d_adam, int apply_update, cudaStream_t s);  // d_adam: DEVICE pointer
-// conv0 backward on tcgen05 (conv0_tc.cu): weights fp32 OIHW [64][3][3][3] -> bf16 [32 (ky,kx,c; 27 used)][64 co];
+// conv0 backward on wgmma (conv0_tc.cu): weights fp32 OIHW [64][3][3][3] -> bf16 [32 (ky,kx,c; 27 used)][64 co];
 // the kernel updates the interior pixels (1x1 GEMM + col2im in smem + Normalize bwd + TV grad + Adam + clamp + EMA)
 int pack_weights_conv0_bwd(const float* w0, bf16* out, cudaStream_t s);
 int launch_conv0_bwd_interior(const bf16* g0, const bf16* w0q, const float* gtv, float* img, float* exp_avg,
@@ -74,7 +74,7 @@ int launch_sse(const bf16* a, const bf16* b, long n, float* partials, int* n_par
 // 2 clamp to [0,1]  (warm start of a scale, ST:285-295, 420)
 int launch_resize(const float* in, int C, int H, int W, float* out, int Ho, int Wo, int mode, int post, cudaStream_t s);
 
-// ---------------------------------------------------------------- Gram / channel sums on tcgen05 (gram_tc.cu)
+// ---------------------------------------------------------------- Gram / channel sums on wgmma (gram_tc.cu)
 int gram_num_splits(long P, int C);
 size_t gram_partials_floats(long P, int C);
 size_t gram_max_partials_floats(int C);  // bound of gram_partials_floats over every P (what the workspace reserves)

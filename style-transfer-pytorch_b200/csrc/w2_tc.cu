@@ -1,21 +1,21 @@
-// Wasserstein-2 style loss on the five tap covariances, forward and backward, at fp32 accuracy on tcgen05:
-//   StyleLossW2.__init__/forward      /root/reference/style_transfer/style_transfer.py:149-181  (ST)
-//   sqrtm_ns (12 Newton-Schulz its)   /root/reference/style_transfer/sqrtm.py:9-25              (SQ)
+// Wasserstein-2 style loss on the five tap covariances, forward and backward, at fp32 accuracy on wgmma:
+//   StyleLossW2.__init__/forward      style_transfer/style_transfer.py:149-181 of the reference  (ST)
+//   sqrtm_ns (12 Newton-Schulz its)   style_transfer/sqrtm.py:9-25 of the reference              (SQ)
 //   _MatrixSquareRootNSLyap.backward  SQ:36-47 (iterative Lyapunov solve, 12 its)
 // plus the closed-form backward of ST:163-181 down to  G = d loss / d srm  and  d loss / d mean.
 //
 // The loss is a cancellation (tr(St + S - 2 sqrt(.)), SURVEY.md section 7.2): plain TF32/bf16 operands are not
 // accurate enough.  Every C x C matrix of the chain therefore lives as TWO fp32 planes, x = hi + lo, where hi has its
 // low 13 mantissa bits cleared (exactly representable in TF32) and lo = x - hi; a product is evaluated as
-//     a*b ~= lo_a*hi_b + hi_a*lo_b + hi_a*hi_b        (3 x tcgen05.mma kind::tf32, fp32 accumulate in TMEM),
+//     a*b ~= lo_a*hi_b + hi_a*lo_b + hi_a*hi_b        (3 x wgmma tf32, fp32 accumulate in registers),
 // the dropped lo*lo term being 2^-22 relative.  The split of a result is done by the producing GEMM's epilogue, so a
 // GEMM only ever streams ready-made planes through TMA.
 //
 // All five layers advance in lock-step: one "round" = one grouped launch whose CTAs are 128 x 64 output tiles of
-// every layer's GEMM (75 or 150 CTAs, largest matrices first).  Both tcgen05 operands are K-major SW128 tiles:
+// every layer's GEMM (75 or 150 tiles, largest matrices first).  Both wgmma operands are K-major SW128 tiles:
 // A[m][k] from the row-major planes of A, B[n][k] from the planes of B^T -- every matrix that is later used as a
 // right factor is therefore written TWICE by its producer: the planes of D (TMA store of the staged tile) and the
-// planes of D^T (scalar stores, coalesced across the warp because TMEM lane = row).
+// planes of D^T (scalar stores).
 //
 // The products are formed in exactly the reference's order, Y <- Y T, Z <- T Z, and NOTHING is symmetrised, although
 // every matrix here is symmetric in exact arithmetic.  Two shortcuts were tried and measured to break parity on real
@@ -44,23 +44,14 @@ namespace {
 
 constexpr int TM = 128, TN = 64, TKF = 32;      // tile rows / cols, k floats per stage (128 B swizzle row)
 constexpr int T_STAGES = 4;
-// TMEM: T_MAX_ACC hi*hi accumulators + two for the cross terms (lo*hi and hi*lo apart), 64 columns each.  The k-steps
-// are dealt to the hi*hi accumulators ROUND-ROBIN: each still sums n_steps / T_MAX_ACC products (short truncating
-// chains, section 5 of DESIGN.md), but consecutive MMAs never target the same accumulator -- a tcgen05.mma that
-// accumulates into the tile its predecessor is still writing waits for it (measured: ~125 cycles per MMA in dependent
-// order vs the 32 its math takes).
-constexpr int T_MAX_ACC = 6;
-constexpr int T_TMEM_COLS = 512;
-constexpr int T_CROSS_COL = T_MAX_ACC * TN;        // lo*hi at T_CROSS_COL, hi*lo at T_CROSS_COL + TN
 constexpr int A_PLANE_BYTES = TM * 128;          // 16 KiB
 constexpr int B_PLANE_BYTES = TN * 128;          // 8 KiB
 constexpr int T_STAGE_BYTES = 2 * A_PLANE_BYTES + 2 * B_PLANE_BYTES;  // A_hi, A_lo, B_hi, B_lo = 48 KiB
 constexpr int T_OFF_BAR = T_STAGES * T_STAGE_BYTES;
-constexpr int T_OFF_TMEMPTR = T_OFF_BAR + (2 * T_STAGES + 1) * 8;
-constexpr int T_OFF_RED = T_OFF_TMEMPTR + 16;
+constexpr int T_OFF_RED = T_OFF_BAR + 2 * T_STAGES * 8;
 constexpr int T_SMEM_BYTES = T_OFF_RED + 64 + 1024;
-constexpr int T_EPI_THREADS = 256;                 // two epilogue groups of four warps: one per 32-column half of the tile
-constexpr int T_THREADS = 64 + T_EPI_THREADS;
+constexpr int T_EPI_THREADS = 256;                 // two consumer warpgroups: rows 0..63 and 64..127 of the tile
+constexpr int T_THREADS = T_EPI_THREADS + 32;      // + the TMA producer warp
 constexpr int NRED = 128;  // max reduction partials per layer
 constexpr int NB = 128;    // helper-kernel CTAs per layer: they are latency-bound element-wise passes (32 CTAs: 48 us)
 static_assert(NB <= NRED, "the covariance kernel writes one partial per CTA");
@@ -120,8 +111,16 @@ __device__ __forceinline__ unsigned ld_acquire_gpu_u32(const unsigned* p) {
 
 // The whole chain of rounds [r0, r1) in ONE persistent, cooperatively launched kernel: one CTA per SM, tile t of a
 // round goes to CTA t % gridDim.x, a grid-wide barrier separates two rounds.  Replaces 24-26 dependent launches per
-// phase: barrier init, TMEM allocation and the launch / drain latency of a grid are paid once, a round boundary costs
-// one atomic + one acquire spin (~1.5 us instead of ~4 us of launch gap).  The arithmetic of a tile is unchanged.
+// phase: barrier init and the launch / drain latency of a grid are paid once, a round boundary costs one atomic + one
+// acquire spin instead of a launch gap.  The arithmetic of a tile is unchanged.
+//
+// Roles: warp 8 TMA producer (four planes per stage), warps 0-7 two consumer warpgroups (tile rows 64 g .. 64 g + 63).
+// A consumer issues per stage 4 k-steps x 3 split products, one k-step per MMA group: the cross terms lo*hi and hi*lo
+// into one accumulator over the whole K range, the hi*hi product into a fresh accumulator that is added into the
+// running sum in round-to-nearest fp32 once the group completes.  The tensor core
+// aligns every product to the accumulator and truncates, so a chain of hi*hi products loses ~2^-25 per step of the
+// sum, systematically, which the Newton-Schulz iteration turns into a bias of the style terms on the ill-conditioned
+// covariances (measured: 1.5e-3 on the 64-channel term with chains of four).
 __global__ void __launch_bounds__(T_THREADS, 1)
 w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __restrict__ grid_counter,
                 unsigned long long* __restrict__ trace) {
@@ -139,25 +138,19 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + T_OFF_BAR);
   uint64_t* empty = full + T_STAGES;
-  uint64_t* t_full = empty + T_STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + T_OFF_TMEMPTR);
   float* s_red = reinterpret_cast<float*>(smem + T_OFF_RED);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < T_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(t_full, 1);
+  if (warp == 8 && lane == 0) {
+    // empty: one arrival per consumer warp once its wgmma reads of the stage are complete
+    for (int i = 0; i < T_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<T_TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  // pipeline ring state, persistent across tiles and rounds (the producer and the MMA warp advance identically)
+  // pipeline ring state, persistent across tiles and rounds (the producer and the consumers advance identically)
   int s = 0;
-  uint32_t ph = 0, tile_parity = 0;
+  uint32_t ph = 0;
   unsigned barriers_done = 0;
 
   // The tile -> CTA map is static, so everything a CTA needs for its first tile of the NEXT round (problem record,
@@ -192,9 +185,8 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
       const int n = pr.n;
       const int k_elems = pr.in_half ? 2 * TKF : TKF;          // elements per 128-byte stage row
       const int n_k = n / k_elems;
-      const int k_steps = n / (pr.in_half ? 16 : 8);           // MMA K steps of the whole tile
 
-      if (warp == 0) {
+      if (warp == 8) {
         // ---- TMA producer: four planes per stage
         const bool leader = elect_one();   // every lane walks the ring state, the elected one issues
         if (leader && first) stamp(round, 0);
@@ -211,147 +203,103 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
           if (++s == T_STAGES) { s = 0; ph ^= 1; }
         }
         __syncwarp();
-      } else if (warp == 1) {
-        // ---- MMA issuer: 4 k-steps (K = 8) x 3 split products per stage.  The tensor core aligns every product to
-        // the accumulator and truncates, so a chain of m products loses ~2^-25 * m of the sum, systematically; on the
-        // ill-conditioned covariances of real activations the Newton-Schulz iteration turns that into a -1e-3 bias of
-        // the style terms (measured).  hi*hi therefore runs in short chains: the n/8 k-steps are dealt out in equal
-        // runs to seven TMEM accumulators (2 steps each at C = 64 ... 10 at C = 512), the small cross terms go to an
-        // eighth, and the epilogue adds all of them in round-to-nearest fp32.
-        constexpr uint32_t idesc = umma_idesc_tf32(TM, TN);
-        constexpr uint32_t idesc_h = umma_idesc_f16(TM, TN);
-        constexpr uint32_t dhi = umma_desc_hi_sw128(1024);
-        const bool leader = elect_one();
+      } else {
+        // ---- consumers: MMA (warpgroup g = rows 64 g .. 64 g + 63 of the tile), then the epilogue
+        const int g = warp >> 2, wq = warp & 3;
         const bool half_in = pr.in_half != 0;
+        float hh[32], cross[32], tot[32];
+#pragma unroll
+        for (int e = 0; e < 32; ++e) tot[e] = 0.f;
         for (int k = 0; k < n_k; ++k) {
           mbar_wait(&full[s], ph);
-          tc_fence_after();
-          if (leader && first && k == 0) stamp(round, 1);
-          if (leader) {
-            const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
-            const uint32_t a_h = umma_desc_lo(base), a_l = umma_desc_lo(base + A_PLANE_BYTES);
-            const uint32_t b_h = umma_desc_lo(base + 2 * A_PLANE_BYTES);
-            const uint32_t b_l = umma_desc_lo(base + 2 * A_PLANE_BYTES + B_PLANE_BYTES);
+          if (threadIdx.x == 0 && first && k == 0) stamp(round, 1);
+          const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
+          const uint64_t a_h = gmma_desc_k(base + g * 64 * 128), a_l = gmma_desc_k(base + A_PLANE_BYTES + g * 64 * 128);
+          const uint64_t b_h = gmma_desc_k(base + 2 * A_PLANE_BYTES);
+          const uint64_t b_l = gmma_desc_k(base + 2 * A_PLANE_BYTES + B_PLANE_BYTES);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {  // 8 floats / 16 halfs = 32 bytes per K step -> +2 in the descriptor
+            wgmma_fence();
             if (!half_in) {
-#pragma unroll
-              for (int kk = 0; kk < TKF / 8; ++kk) {  // 8 floats = 32 bytes per K step -> +2 in the descriptor
-                const int step = k * (TKF / 8) + kk;
-                const uint32_t t_main = tmem_base + (step % T_MAX_ACC) * TN, t_cross = tmem_base + T_CROSS_COL;
-                umma_tf32_split(t_cross, a_l + 2 * kk, dhi, b_h + 2 * kk, dhi, idesc, step > 0);
-                umma_tf32_split(t_main, a_h + 2 * kk, dhi, b_h + 2 * kk, dhi, idesc, step >= T_MAX_ACC);
-                umma_tf32_split(t_cross + TN, a_h + 2 * kk, dhi, b_l + 2 * kk, dhi, idesc, step > 0);
-              }
+              wgmma_tf32(cross, a_l + 2 * kk, b_h + 2 * kk, k > 0 || kk > 0);
+              wgmma_tf32(hh, a_h + 2 * kk, b_h + 2 * kk, 0);
+              wgmma_tf32(cross, a_h + 2 * kk, b_l + 2 * kk, 1);
             } else {
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {        // 16 halfs = 32 bytes per K step -> +2 in the descriptor
-                const int step = k * 4 + kk;
-                const uint32_t t_main = tmem_base + (step % T_MAX_ACC) * TN, t_cross = tmem_base + T_CROSS_COL;
-                umma_bf16_split(t_cross, a_l + 2 * kk, dhi, b_h + 2 * kk, dhi, idesc_h, step > 0);
-                umma_bf16_split(t_main, a_h + 2 * kk, dhi, b_h + 2 * kk, dhi, idesc_h, step >= T_MAX_ACC);
-                umma_bf16_split(t_cross + TN, a_h + 2 * kk, dhi, b_l + 2 * kk, dhi, idesc_h, step > 0);
-              }
+              wgmma_f16<0, 0>(cross, a_l + 2 * kk, b_h + 2 * kk, k > 0 || kk > 0);
+              wgmma_f16<0, 0>(hh, a_h + 2 * kk, b_h + 2 * kk, 0);
+              wgmma_f16<0, 0>(cross, a_h + 2 * kk, b_l + 2 * kk, 1);
             }
-            umma_commit(&empty[s]);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(hh);
+#pragma unroll
+            for (int e = 0; e < 32; ++e) tot[e] += hh[e];
           }
-          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[s]);
           if (++s == T_STAGES) { s = 0; ph ^= 1; }
         }
-        if (leader) umma_commit(t_full);
-        __syncwarp();
-      } else {
-        // ---- epilogue (2 groups x 128 threads, TMEM lane = tile row; group g drains columns [32 g, 32 g + 32))
-        const int wq = warp & 3;
-        const int grp = (warp - 2) >> 2;
-        const bool issuer = warp == 2 && lane == 0;   // the one thread that issues the TMA stores / writes the partials
-        const int r = wq * 32 + lane;
-        const int gi = ti * TM + r;
+        wgmma_fence_acc(cross);
+        // every consumer is done reading the pipeline buffers, which the epilogue reuses as staging
+        named_bar_sync(2, T_EPI_THREADS);
+        const bool issuer = threadIdx.x == 0;   // the one thread that issues the TMA stores / writes the partials
+        if (issuer && first) stamp(round, 2);
         const size_t nn = (size_t)n * n;
         uint8_t* stg = smem + STG_OFF;
-        mbar_wait(t_full, tile_parity);
-        tc_fence_after();
-        if (issuer && first) stamp(round, 2);
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16);
-        const int n_chunks = k_steps < T_MAX_ACC ? k_steps : T_MAX_ACC;   // hi*hi accumulators in use
-        const bool valid = gi < n;
         const float cross_scale = pr.in_half ? H_LO_INV : 1.f;   // fp16 pairs keep the residual plane times 2^11
         const bool half_out = pr.out_half != 0;
         __half* Dh = reinterpret_cast<__half*>(pr.D);
+        const int cq = 2 * (lane & 3);
         float ssq = 0.f, tr = 0.f;
-        {
-          const int h = grp;
-          uint32_t v[32], v2[32];
-          float acc[32];
-          // chunk sums in the same order as ever (c = 0, 1, 2, ...); the TMEM loads go out in pairs under one wait
-          tmem_ld_32x32(taddr + h * 32, v);
-          if (n_chunks > 1) tmem_ld_32x32(taddr + TN + h * 32, v2);
-          tmem_ld_wait();
 #pragma unroll
-          for (int e = 0; e < 32; ++e) acc[e] = __uint_as_float(v[e]);
-          if (n_chunks > 1) {
+        for (int hr = 0; hr < 2; ++hr) {
+          const int r = 64 * g + 16 * wq + (lane >> 2) + 8 * hr;   // tile row
+          const int gi = ti * TM + r;
+          const bool valid = gi < n;
 #pragma unroll
-            for (int e = 0; e < 32; ++e) acc[e] += __uint_as_float(v2[e]);
-          }
-          for (int c = 2; c < n_chunks; c += 2) {
-            tmem_ld_32x32(taddr + c * TN + h * 32, v);
-            if (c + 1 < n_chunks) tmem_ld_32x32(taddr + (c + 1) * TN + h * 32, v2);
-            tmem_ld_wait();
+          for (int q = 0; q < 8; ++q) {
+            const int c = 8 * q + cq;                              // tile column (and c + 1)
+            float o[2];
 #pragma unroll
-            for (int e = 0; e < 32; ++e) acc[e] += __uint_as_float(v[e]);
-            if (c + 1 < n_chunks) {
-#pragma unroll
-              for (int e = 0; e < 32; ++e) acc[e] += __uint_as_float(v2[e]);
+            for (int e = 0; e < 2; ++e) {
+              const int idx = 4 * q + 2 * hr + e;
+              o[e] = (tot[idx] + cross[idx] * cross_scale) * pr.alpha;
+              if (gi == tj * TN + c + e) { o[e] += pr.gamma; tr += o[e]; }
+              if (valid) ssq = fmaf(o[e], o[e], ssq);
             }
-          }
-          tmem_ld_32x32(taddr + T_CROSS_COL + h * 32, v);
-          tmem_ld_32x32(taddr + T_CROSS_COL + TN + h * 32, v2);
-          tmem_ld_wait();
+            const int gj = tj * TN + c;
+            if (!half_out) {
+              // planes of column half h = c / 32: [128 rows][32 floats], 128-byte swizzle as the TMA store expects
+              const int h = c >> 5, cc = c & 31;
+              uint8_t* row_hi = stg + (h * 2) * A_PLANE_BYTES + r * 128;
+              uint8_t* row_lo = row_hi + A_PLANE_BYTES;
+              const int off = (((cc >> 2) ^ (r & 7)) << 4) + (cc & 3) * 4;
+              float vh[2], vl[2];
+              split_tf32(o[0], vh[0], vl[0]);
+              split_tf32(o[1], vh[1], vl[1]);
+              *reinterpret_cast<float2*>(row_hi + off) = make_float2(vh[0], vh[1]);
+              *reinterpret_cast<float2*>(row_lo + off) = make_float2(vl[0], vl[1]);
+              if (pr.write_t && valid) {  // D^T planes
 #pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(v2[e]));
-          const int gj0 = tj * TN + h * 32;
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {   // finished values of this row's 32 columns
-            float o = (acc[e] + __uint_as_float(v[e]) * cross_scale) * pr.alpha;
-            if (gi == gj0 + e) { o += pr.gamma; tr += o; }
-            if (valid) ssq = fmaf(o, o, ssq);
-            acc[e] = o;
-          }
-          if (!half_out) {
-            uint8_t* row_hi = stg + (h * 2) * A_PLANE_BYTES + r * 128;
-            uint8_t* row_lo = row_hi + A_PLANE_BYTES;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              float vh[4], vl[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) split_tf32(acc[4 * q + e], vh[e], vl[e]);
-              const int chunk = (q ^ (r & 7)) * 16;  // 128-byte swizzle, as the TMA store expects
-              *reinterpret_cast<float4*>(row_hi + chunk) = make_float4(vh[0], vh[1], vh[2], vh[3]);
-              *reinterpret_cast<float4*>(row_lo + chunk) = make_float4(vl[0], vl[1], vl[2], vl[3]);
-              if (pr.write_t && valid) {  // D^T planes: for a fixed column the 32 lanes (consecutive rows) write 128 B
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const size_t at = 2 * nn + (size_t)(gj0 + 4 * q + e) * n + gi;
+                for (int e = 0; e < 2; ++e) {
+                  const size_t at = 2 * nn + (size_t)(gj + e) * n + gi;
                   pr.D[at] = vh[e];
                   pr.D[nn + at] = vl[e];
                 }
               }
-            }
-          } else {
-            // fp16 pair: one 128 x 64 tile per plane (row = 64 halfs = 128 bytes), hi plane at stg, lo plane after it;
-            // this half of the row fills 16-byte chunks 4h .. 4h+3
-            uint8_t* row_hi = stg + r * 128;
-            uint8_t* row_lo = row_hi + A_PLANE_BYTES;
+            } else {
+              // fp16 pair: one 128 x 64 tile per plane (row = 64 halfs = 128 bytes), hi plane at stg, lo plane after it
+              uint8_t* row_hi = stg + r * 128;
+              uint8_t* row_lo = row_hi + A_PLANE_BYTES;
+              const int off = ((q ^ (r & 7)) << 4) + cq * 2;
+              __half hh[2], ll[2];
+              split_half(o[0], hh[0], ll[0]);
+              split_half(o[1], hh[1], ll[1]);
+              *reinterpret_cast<__half2*>(row_hi + off) = __halves2half2(hh[0], hh[1]);
+              *reinterpret_cast<__half2*>(row_lo + off) = __halves2half2(ll[0], ll[1]);
+              if (pr.write_t && valid) {  // D^T planes
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              __half hh[8], ll[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) split_half(acc[8 * q + e], hh[e], ll[e]);
-              const int chunk = ((h * 4 + q) ^ (r & 7)) * 16;
-              *reinterpret_cast<uint4*>(row_hi + chunk) = *reinterpret_cast<const uint4*>(hh);
-              *reinterpret_cast<uint4*>(row_lo + chunk) = *reinterpret_cast<const uint4*>(ll);
-              if (pr.write_t && valid) {  // D^T planes: for a fixed column the 32 lanes write 64 contiguous bytes
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                  const size_t at = 2 * nn + (size_t)(gj0 + 8 * q + e) * n + gi;
+                for (int e = 0; e < 2; ++e) {
+                  const size_t at = 2 * nn + (size_t)(gj + e) * n + gi;
                   Dh[at] = hh[e];
                   Dh[nn + at] = ll[e];
                 }
@@ -359,7 +307,6 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
             }
           }
         }
-        tc_fence_before();
         fence_proxy_async_smem();
         // the D^T planes were written through the generic proxy; the next round reads them through TMA (async proxy)
         asm volatile("fence.proxy.async;" ::: "memory");
@@ -382,7 +329,7 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
         if (pr.red_out != nullptr) {
           ssq = warp_sum(ssq);
           tr = warp_sum(tr);
-          if (lane == 0) { s_red[(grp * 4 + wq) * 2] = ssq; s_red[(grp * 4 + wq) * 2 + 1] = tr; }
+          if (lane == 0) { s_red[warp * 2] = ssq; s_red[warp * 2 + 1] = tr; }
           named_bar_sync(1, T_EPI_THREADS);
           if (issuer) {
             const int ntj = n / TN;
@@ -397,11 +344,8 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
           if (first) stamp(round, 4);
         }
       }
-      // ---- end of tile: TMEM drained, staging smem free, every role done
-      tc_fence_before();
+      // ---- end of tile: staging smem free, every role done
       __syncthreads();
-      tc_fence_after();
-      tile_parity ^= 1;
     }
     // ---- grid-wide barrier between two rounds (the last round of the launch ends with the kernel)
     if (round + 1 < r1) {
@@ -426,9 +370,6 @@ w2_chain_kernel(const W2Round* __restrict__ rounds, int r0, int r1, unsigned* __
       __syncthreads();
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<T_TMEM_COLS>(tmem_base);
 }
 
 // ---- helpers: grid (5 layers, NB CTAs), 256 threads; reductions via fixed-order partials (deterministic)
@@ -745,7 +686,7 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
       for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.T, L.Z[s], L.Y[s], -0.5f, 1.5f); }
       end_round();
       begin_round();
-      for (int l = 4; l >= 0; --l) {  // largest matrices first: the two CTAs beyond 148 are short ones
+      for (int l = 4; l >= 0; --l) {  // largest matrices first: the tiles beyond one per SM are short ones
         W2Layer& L = host_layers[l];
         b.add(L.n, L.Y[d], L.Y[s], L.T, 1.f, 0.f, it == 11 ? L.red : nullptr);
         if (it < 11) b.add(L.n, L.Z[d], L.T, L.Z[s], 1.f);  // Z is dead after the last Y

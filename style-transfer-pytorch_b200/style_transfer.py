@@ -1,4 +1,4 @@
-"""Drop-in `StyleTransfer` whose per-iteration body is one call into libstb200 (hand-written sm_100a CUDA).
+"""Drop-in `StyleTransfer` whose per-iteration body is one call into libstb200 (hand-written sm_90a CUDA).
 
 Public surface mirrors /root/reference/style_transfer/style_transfer.py ("ST"): `StyleTransfer(devices, pooling)`
 (ST:310), attributes (ST:311-324), `get_image_tensor` / `get_image` (ST:335-347), `stylize(...)` with the same
@@ -314,12 +314,12 @@ class StyleTransfer:
         if len(self.devices) not in (1, 2):
             raise ValueError('Only 1 or 2 devices are supported.')
         if not torch.cuda.is_available():
-            raise RuntimeError('CUDA is not available; the B200-native hot path cannot run (there is no CPU '
+            raise RuntimeError('CUDA is not available; the H100-native hot path cannot run (there is no CPU '
                                'fallback).')
         if any(d.type != 'cuda' for d in self.devices):
             # the reference's default argument is devices=['cpu'] (ST:310): call sites that rely on it keep working,
             # on the GPU this implementation exists for -- loudly, never on a CPU path
-            warnings.warn('style-transfer-pytorch_b200 runs its hot path only on CUDA (sm_100a) devices; '
+            warnings.warn('style-transfer-pytorch_b200 runs its hot path only on CUDA (sm_90a) devices; '
                           f'devices={[str(d) for d in self.devices]} -> using cuda:{torch.cuda.current_device()} '
                           '(there is no CPU fallback)')
             self.devices = [torch.device('cuda', torch.cuda.current_device())]

@@ -10,7 +10,7 @@ for _p in (str(ROOT), str(Path(__file__).resolve().parent)):
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a real B200 (run with -m gpu on the GPU box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA GPU (an H100; run with -m gpu on a GPU machine)')
 
 
 def pytest_collection_modifyitems(config, items):

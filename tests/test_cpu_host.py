@@ -49,8 +49,10 @@ def test_product_does_not_touch_the_oracle():
         assert 'st_oracle' not in txt and 'libst_oracle' not in txt and 'reference_harness' not in txt, p
 
 
-def test_no_cpu_fallback():
+def test_no_cpu_fallback(monkeypatch):
+    import torch
     import style_transfer_b200 as stb
+    monkeypatch.setattr(torch.cuda, 'is_available', lambda: False)   # a host without CUDA, also on a GPU machine
     with pytest.raises(RuntimeError):
         stb.StyleTransfer(devices=['cpu'])
     with pytest.raises(ValueError):

@@ -119,7 +119,7 @@ def test_conv0_tv_forward_and_backward(G, H, W):
     torch.cuda.synchronize()
     acts0 = {1: torch.ones(1, 64, H, W, dtype=torch.float64)}  # mask already applied in g0
     ref = O.vgg_backward({1: G.nchw(g0).double()}, acts0, [(w0.double(), b0.double())], 'max')
-    # interior pixels come from the tcgen05 dgrad with bf16 weights and a bf16 result (2^-9 relative), the border
+    # interior pixels come from the wgmma dgrad with bf16 weights and a bf16 result (2^-9 relative), the border
     # ring (replicate-pad adjoint) is evaluated in fp32
     assert G.rel_err(grad, ref.float()) < 6e-3
     ring = torch.ones(1, 3, H, W, dtype=torch.bool)

@@ -82,7 +82,7 @@ def test_size_helpers():
 
 
 def test_goldens_are_what_the_live_reference_produces(vgg_weights):
-    """Where the reference tree is present (build container: /root/reference, or the baseline/_ref install), re-run the
+    """Where build() copied the reference modules into oracle/_ref (wherever a reference checkout is present), re-run the
     UNMODIFIED reference for one case and compare with the committed golden: the fixtures are not hand-edited and the
     installed torch still reproduces them.  Skipped where no reference is available."""
     from oracle import reference_harness as RH

@@ -1,4 +1,4 @@
-"""GPU bring-up check for the tcgen05 pixel-GEMM kernel (run under gpurun).  Compares against torch fp32 conv2d
+"""GPU bring-up check for the wgmma pixel-GEMM kernel.  Compares against torch fp32 conv2d
 on bf16-rounded operands and times the VGG layer shapes at 2048^2.  Not a pytest file: prints diagnostics."""
 import ctypes
 import sys

@@ -1,6 +1,6 @@
 """Library bar (SURVEY.md section 8d): the UNMODIFIED reference's own --devices cuda:0 path (cuDNN / cuBLAS, TF32 off by
 torch default for matmul, cuDNN conv TF32 on) timed on the same synthetic workload as bench.py.
-Needs the reference install under baseline/_ref (see DESIGN.md).  Usage: python tools/ref_gpu_bench.py [size] [iters]"""
+Needs the reference modules under oracle/_ref (copied by build() where a reference checkout is present).  Usage: python tools/ref_gpu_bench.py [size] [iters]"""
 import json
 import sys
 from pathlib import Path

@@ -1,6 +1,6 @@
 """Wave-quantised cost model of the twelve 3x3 convolutions (forward + dgrad) of one tiled rank, relative to 1/N of the
-untiled run (DESIGN.md section 6).  A conv launch is `tiles` CTA tiles of 16 x (8 MT) pixels x BN channels walked by 148
-persistent CTAs, so its time is ceil(tiles / 148) waves of one tile time.
+untiled run (DESIGN.md section 6).  A conv launch is `tiles` CTA tiles of 16 x (8 MT) pixels x BN channels walked by 132
+persistent CTAs (one per H100 SM), so its time is ceil(tiles / 132) waves of one tile time.
 
   python tools/tile_model.py [size]
 
@@ -29,7 +29,7 @@ def cost(size, rows_fn, tile_h=16):
             mt = 1 if bn == 256 else 2
             tile_w = (8 if tile_h == 16 else 16) * mt
             tiles = math.ceil(w / tile_w) * math.ceil(rows / tile_h) * (c_out // bn)
-            total += math.ceil(tiles / 148) * 148 * (2 * 9 * c_in * bn * 128 * mt)
+            total += math.ceil(tiles / 132) * 132 * (2 * 9 * c_in * bn * 128 * mt)
     return total
 
 
