@@ -84,10 +84,27 @@ STB_API int stb_set_targets(stb_ctx* ctx, int H, int W, const void* content_targ
 STB_API int stb_iterate(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step,
                         float lr, float beta1, float beta2, float adam_eps, float ema_decay, float* loss_out_host8,
                         void* stream);
-/* closure-only variant (apply_update = 0): loss and d loss/d image (grad_out fp32 NCHW), e.g. for an L-BFGS host. */
+/* closure-only variant (apply_update = 0): loss and d loss/d image (grad_out fp32 NCHW), e.g. for a host optimizer. */
 STB_API int stb_iterate_ex(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step,
                            float lr, float beta1, float beta2, float adam_eps, float ema_decay, int apply_update,
                            float* grad_out, float* loss_out_host8, void* stream);
+
+/* ------------------------------------------------------------------ optimizer='lbfgs' (ST:464-465) on the device
+ * One iteration = closure (forward, losses, backward) + torch.optim.LBFGS.step with lr = 1, max_iter = 1,
+ * history_size = STB_LBFGS_HISTORY, tolerance_grad = 1e-7, tolerance_change = 1e-9 and no line search, followed by
+ * ema = ema * decay + (1 - decay) * img.  There is no clamp on this path (ST:482-485), as in the reference.
+ * The optimizer state (history ring, g, g_prev, d, scalars) is ONE caller-owned device block of
+ * stb_lbfgs_state_bytes(H, W) bytes, 256-byte aligned (~25 x 3HW floats: ~1.26 GB at 2048^2).  The reference builds
+ * a fresh optim.LBFGS per scale: call stb_lbfgs_reset once per scale, before its first iteration.
+ * stb_iterate_lbfgs runs on the targets' H x W (stb_set_targets) and needs a context without a band.  It is one
+ * stream-ordered sequence, replayed as a CUDA graph, with no host sync; the loss of the PRE-step image goes to the loss
+ * ring (stb_set_loss_ring) under the stamp `step`, the running iteration count of the whole stylize() call, and
+ * optionally to loss_out_host8. */
+#define STB_LBFGS_HISTORY 10
+STB_API int stb_lbfgs_state_bytes(int H, int W, size_t* bytes);
+STB_API int stb_lbfgs_reset(void* state, int H, int W, void* stream);
+STB_API int stb_iterate_lbfgs(stb_ctx* ctx, float* img, float* ema, void* state, size_t state_bytes, int64_t step,
+                              float ema_decay, float* loss_out_host8, void* stream);
 
 /* ------------------------------------------------------------------ spatial tiling across GPUs (SURVEY.md 8e)
  * A context may work on a horizontal band (plus halo aprons) of a taller image: H passed to the other calls is the
@@ -158,7 +175,8 @@ STB_API int stb_iterate_banded(stb_ctx* ctx, float* img, float* exp_avg, float* 
 /* 1: iterations replay as CUDA graphs, 2: enabled but nothing captured yet, 0: eager launches (note_out says why). */
 STB_API int stb_graph_status(stb_ctx* ctx, char* note_out, size_t note_bytes);
 /* Kernel launches issued through graph replays so far, counted from the captured graphs: number of replays, kernels
- * they launched, kernel nodes per graph slot {stb_iterate, stb_iterate_fwd, stb_iterate_bwd, stb_iterate_banded}. */
+ * they launched (stb_iterate_lbfgs' replays included), kernel nodes per graph slot {stb_iterate, stb_iterate_fwd,
+ * stb_iterate_bwd, stb_iterate_banded}. */
 STB_API int stb_launch_count(stb_ctx* ctx, int64_t* graph_replays, int64_t* kernels_replayed, int* kernels_per_graph4);
 
 /* ------------------------------------------------------------------ measurement (bench.py roofline leg)

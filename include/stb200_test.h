@@ -38,6 +38,11 @@ STB_API int stb_test_w2(const float* mean_t, const float* srm_t, const float* S_
                         float npix, float weight, void* ws, size_t ws_bytes, float* loss_out, float* gs_out,
                         float* gmu_out, float* csqrt_out, void* stream);
 STB_API size_t stb_test_w2_workspace_bytes(void);
+/* the L-BFGS step of stb_iterate_lbfgs alone (closure replaced by a given gradient, grad NULL: the gradient already held
+ * by the state): state of stb_lbfgs_state_bytes(H, W) bytes, x / ema fp32 [3*H*W].  pairs_out / t_out (optional; the
+ * call then synchronises the stream): history pairs held and step length of the current direction. */
+STB_API int stb_test_lbfgs_step(void* state, size_t bytes, int H, int W, float* x, const float* grad, float* ema,
+                                float ema_decay, int* pairs_out, float* t_out, void* stream);
 
 #ifdef __cplusplus
 }

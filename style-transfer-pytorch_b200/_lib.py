@@ -44,6 +44,9 @@ def _declare(lib):
         'stb_set_targets': [vp, i, i, vp, f, pp, pp, C.POINTER(f), f, f, vp],
         'stb_iterate': [vp, vp, vp, vp, vp, i64, f, f, f, f, f, vp, vp],
         'stb_iterate_ex': [vp, vp, vp, vp, vp, i64, f, f, f, f, f, i, vp, vp, vp],
+        'stb_lbfgs_state_bytes': [i, i, C.POINTER(sz)],
+        'stb_lbfgs_reset': [vp, i, i, vp],
+        'stb_iterate_lbfgs': [vp, vp, vp, vp, sz, i64, f, vp, vp],
         'stb_set_band': [vp, i, i, i, i],
         'stb_stats_block': [vp, i, i, pp, C.POINTER(sz)],
         'stb_iterate_fwd': [vp, vp, vp],
@@ -86,6 +89,7 @@ def _declare_test(lib):
         'stb_test_pool_bwd': [i, vp, vp, vp, i, i, i, vp],
         'stb_test_gram': [vp, C.c_long, i, vp, sz, vp, vp, vp],
         'stb_test_w2': [vp, vp, vp, vp, i, f, f, vp, sz, vp, vp, vp, vp, vp],
+        'stb_test_lbfgs_step': [vp, sz, i, i, vp, vp, vp, f, C.POINTER(i), C.POINTER(f), vp],
     })
     lib.stb_test_gram_partials_floats.argtypes = [C.c_long, i]
     lib.stb_test_gram_partials_floats.restype = sz
@@ -97,6 +101,7 @@ def _declare_test(lib):
 EXPORTS = [
     'stb_last_error', 'stb_ctx_create', 'stb_ctx_destroy', 'stb_workspace_bytes', 'stb_bind_workspace',
     'stb_style_stats', 'stb_content_features', 'stb_set_targets', 'stb_iterate', 'stb_iterate_ex',
+    'stb_lbfgs_state_bytes', 'stb_lbfgs_reset', 'stb_iterate_lbfgs',
     'stb_set_band', 'stb_stats_block', 'stb_iterate_fwd', 'stb_iterate_bwd', 'stb_adam_update',
     'stb_set_loss_ring', 'stb_resize', 'stb_comm_create', 'stb_comm_connect_ipc', 'stb_comm_connect_local', 'stb_comm_disconnect', 'stb_comm_alloc_workspace',
     'stb_comm_connect_ws_ipc', 'stb_comm_connect_ws_local', 'stb_comm_release_workspace',
@@ -107,7 +112,7 @@ EXPORTS = [
 TEST_EXPORTS = [
     'stb_test_last_error', 'stb_pack_weights', 'stb_test_pixel_gemm', 'stb_test_conv0_fwd', 'stb_test_conv0_bwd',
     'stb_test_conv_pool', 'stb_test_pool_bwd', 'stb_test_gram', 'stb_test_gram_partials_floats', 'stb_test_w2',
-    'stb_test_w2_workspace_bytes',
+    'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step',
 ]
 
 

@@ -113,7 +113,9 @@ struct stb_ctx {
       exec = nullptr; key = GraphKey{}; hits = 0; kernel_nodes = 0;
     }
   };
-  GraphSlot gslot[4];  // 0: stb_iterate, 1: stb_iterate_fwd, 2: stb_iterate_bwd (host-driven phases), 3: stb_iterate_banded
+  // 0: stb_iterate, 1: stb_iterate_fwd, 2: stb_iterate_bwd (host-driven phases), 3: stb_iterate_banded,
+  // 4: stb_iterate_lbfgs
+  GraphSlot gslot[5];
   void reset_graphs() { for (auto& g : gslot) g.reset(); }
   bool graphs_enabled = true;
   std::string graph_note;  // why graph replay was switched off for this context (stb_graph_status)
@@ -381,6 +383,9 @@ AdamScalars make_adam_scalars(int64_t step, float lr, float beta1, float beta2, 
   return as;
 }
 
+// the iteration counter of the loss ring's stamps on a path without Adam scalars (stb_iterate_lbfgs)
+__global__ void advance_step_kernel(long long* step) { *step += 1; }
+
 __global__ void scale_copy_kernel(const float* __restrict__ in, float* __restrict__ out, long n, float scale) {
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
     out[i] = in[i] * scale;
@@ -646,7 +651,7 @@ int iterate_fwd(stb_ctx* ctx, const Plan& pl, const float* img, cudaStream_t s, 
 // phase 2: W2 losses on the (globally reduced) statistics, backward to the image, optional fused update
 int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, float* exp_avg, float* exp_avg_sq, float* ema,
                 const AdamScalars* d_adam, int apply_update, float* grad_out, float* loss_out_host8, cudaStream_t s,
-                const HaloPlans* halo = nullptr) {
+                const HaloPlans* halo = nullptr, bool publish_loss = false) {
   const int H = pl.H, W = pl.W;
   const long n22 = (long)band_rows(ctx, pl, kContentConv).h_global * pl.w[kContentConv] * 512;  // global numel
   float* loss_dev = at<float>(ctx, pl.loss_off);
@@ -658,7 +663,8 @@ int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, float* exp_avg, float*
   ctx->prof.begin(PC_FINALIZE, s);
   finalize_loss_kernel<<<1, 32, 0, s>>>(at<float>(ctx, pl.stats_off) + pl.stats_scalars,
                                         ctx->content_weight / (float)n22, loss_dev + 16, ctx->tv_weight, loss_dev,
-                                        apply_update || ctx->band_on ? ctx->ring_dev : nullptr, ctx->ring_slots,
+                                        apply_update || ctx->band_on || publish_loss ? ctx->ring_dev : nullptr,
+                                        ctx->ring_slots,
                                         ctx->d_step);
   ctx->prof.end(s);
   if (loss_out_host8)
@@ -926,6 +932,57 @@ int stb_iterate(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, flo
                 float beta1, float beta2, float adam_eps, float ema_decay, float* loss_out_host8, void* stream) {
   return stb_iterate_ex(ctx, img, exp_avg, exp_avg_sq, ema, step, lr, beta1, beta2, adam_eps, ema_decay, 1, nullptr,
                         loss_out_host8, stream);
+}
+
+// ---- optimizer='lbfgs' (ST:464-465, SURVEY.md 8f row 4): closure + the L-BFGS step of lbfgs.cu + EMA, one graph
+int stb_lbfgs_state_bytes(int H, int W, size_t* bytes) {
+  STB_CHECK(bytes != nullptr && H > 0 && W > 0, STB_ERR_INVALID, "bad argument");
+  *bytes = lbfgs_state_bytes(3l * H * W);
+  return STB_OK;
+}
+
+int stb_lbfgs_reset(void* state, int H, int W, void* stream) {
+  STB_CHECK(state != nullptr && H > 0 && W > 0, STB_ERR_INVALID, "bad argument");
+  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0, STB_ERR_INVALID, "L-BFGS state must be 256-byte aligned");
+  return launch_lbfgs_reset(state, static_cast<cudaStream_t>(stream));
+}
+
+int stb_iterate_lbfgs(stb_ctx* ctx, float* img, float* ema, void* state, size_t state_bytes, int64_t step,
+                      float ema_decay, float* loss_out_host8, void* stream) {
+  STB_CHECK(ctx && img && ema && state, STB_ERR_INVALID, "null argument");
+  STB_ENTER(ctx);
+  STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede stb_iterate_lbfgs");
+  STB_CHECK(!ctx->band_on, STB_ERR_STATE, "L-BFGS runs on the whole image: the context has a band set");
+  STB_CHECK(step >= 1, STB_ERR_INVALID, "step must be >= 1");
+  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(ema) & 15) == 0,
+            STB_ERR_INVALID, "state must be 256-byte aligned, img and ema 16-byte aligned");
+  const long n = 3l * ctx->tH * ctx->tW;
+  STB_CHECK(state_bytes >= lbfgs_state_bytes(n), STB_ERR_INVALID,
+            "L-BFGS state of %zu bytes is too small for %dx%d (needs %zu)", state_bytes, ctx->tH, ctx->tW,
+            lbfgs_state_bytes(n));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  Plan pl;
+  make_plan(ctx, ctx->tH, ctx->tW, &pl);
+  STB_TRY(ensure_ws(ctx, pl));
+  // the loss ring's stamp is the device step counter, carried across scales like Adam's (stb_iterate_ex)
+  if (ctx->dev_step_mirror != step - 1) {
+    const long long v = step - 1;
+    STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &v, sizeof(v), cudaMemcpyHostToDevice, s));
+    STB_CUDA_CHECK(cudaStreamSynchronize(s));  // `v` is a stack variable; this path runs once per scale at most
+  }
+  ctx->dev_step_mirror = step;
+  float* grad = lbfgs_grad_buffer(state, n);
+  auto run = [&]() -> int {
+    STB_TRY(iterate_fwd(ctx, pl, img, s));
+    advance_step_kernel<<<1, 1, 0, s>>>(ctx->d_step);
+    STB_TRY(iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad, loss_out_host8, s, nullptr, true));
+    return launch_lbfgs_step(state, n, img, ema, ema_decay, s);
+  };
+  stb_ctx::GraphKey key{};
+  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = state; key.ema = ema;
+  key.loss = loss_out_host8; key.decay = ema_decay;
+  return run_graphed(ctx, 4, key, true, s, run);
 }
 
 // Per-kernel-class device timing (CUDA events on the launching stream).  enable: 1 starts recording spans for
@@ -1261,7 +1318,7 @@ int stb_launch_count(stb_ctx* ctx, int64_t* graph_replays, int64_t* kernels_repl
   if (graph_replays) *graph_replays = ctx->graph_replays;
   if (kernels_replayed) *kernels_replayed = ctx->kernels_replayed;
   if (kernels_per_graph4)
-    for (int i = 0; i < 4; ++i) kernels_per_graph4[i] = ctx->gslot[i].kernel_nodes;
+    for (int i = 0; i < 4; ++i) kernels_per_graph4[i] = ctx->gslot[i].kernel_nodes;   // the ABI's four slots
   return STB_OK;
 }
 

@@ -99,6 +99,24 @@ int stb_test_gram(const void* F_bf16, long P, int C, float* partials_ws, size_t 
                      static_cast<cudaStream_t>(stream));
 }
 
+// The launch sequence of the L-BFGS step of stb_iterate_lbfgs on a scripted gradient (NULL: the gradient already in
+// the state, e.g. to time the step alone).  pairs_out / t_out (optional, synchronous): history pairs and step length.
+int stb_test_lbfgs_step(void* state, size_t bytes, int H, int W, float* x, const float* grad, float* ema,
+                        float ema_decay, int* pairs_out, float* t_out, void* stream) {
+  STB_CHECK(state && x && ema && H > 0 && W > 0, STB_ERR_INVALID, "bad argument");
+  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(ema) & 15) == 0,
+            STB_ERR_INVALID, "state must be 256-byte aligned, x and ema 16-byte aligned");
+  const long n = 3l * H * W;
+  STB_CHECK(bytes >= lbfgs_state_bytes(n), STB_ERR_INVALID, "L-BFGS state too small");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (grad)
+    STB_CUDA_CHECK(cudaMemcpyAsync(lbfgs_grad_buffer(state, n), grad, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  STB_TRY(launch_lbfgs_step(state, n, x, ema, ema_decay, s));
+  if (pairs_out || t_out) STB_TRY(lbfgs_read_info(state, pairs_out, t_out, s));
+  return STB_OK;
+}
+
 size_t stb_test_w2_workspace_bytes(void) { return W2Engine::workspace_bytes(); }
 
 // Runs the W2 engine with the given problem placed in the slot of matching size (other slots get a benign

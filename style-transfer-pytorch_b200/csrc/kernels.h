@@ -74,6 +74,17 @@ int launch_sse(const bf16* a, const bf16* b, long n, float* partials, int* n_par
 // 2 clamp to [0,1]  (warm start of a scale, ST:285-295, 420)
 int launch_resize(const float* in, int C, int H, int W, float* out, int Ho, int Wo, int mode, int post, cudaStream_t s);
 
+// ---------------------------------------------------------------- L-BFGS step on the device (lbfgs.cu)
+// torch.optim.LBFGS.step (lr 1, max_iter 1, history STB_LBFGS_HISTORY, no line search) + EMA on n-float vectors; the
+// state is one caller-owned block of lbfgs_state_bytes(n) bytes (256-byte aligned), reset by launch_lbfgs_reset.
+size_t lbfgs_state_bytes(long n);
+float* lbfgs_grad_buffer(void* state, long n);  // where the gradient of the step must be written
+int launch_lbfgs_reset(void* state, cudaStream_t s);
+// fixed launch sequence (capturable): the step on x, then ema = ema * decay + (1 - decay) * x
+int launch_lbfgs_step(void* state, long n, float* x, float* ema, float ema_decay, cudaStream_t s);
+// synchronous read of the pair count and the step length t of the current direction (test hook)
+int lbfgs_read_info(const void* state, int* pairs, float* t, cudaStream_t s);
+
 // ---------------------------------------------------------------- Gram / channel sums on wgmma (gram_tc.cu)
 int gram_num_splits(long P, int C);
 size_t gram_partials_floats(long P, int C);

@@ -617,7 +617,7 @@ class StyleTransfer:
 
         exp_avg = exp_avg_sq = None
         step = 0
-        lbfgs = None
+        lbfgs_state = None
         self._stream.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.device(dev), torch.cuda.stream(self._stream), torch.no_grad():
             for scale in scales:
@@ -704,7 +704,8 @@ class StyleTransfer:
                             stats = self.model.stats_view(h_loc, cw)
                             grad = torch.empty_like(self.image)
                 else:
-                    lbfgs = self._make_lbfgs()
+                    lbfgs_state = None   # hand the previous scale's block back before the new one is allocated
+                    lbfgs_state = self._lbfgs_state(ch, cw)
                 torch.cuda.empty_cache()
 
                 actual_its = initial_iterations if scale == scales[0] else iterations
@@ -716,7 +717,8 @@ class StyleTransfer:
                         step += 1
                         self._iterate(exp_avg, exp_avg_sq, step, step_size, avg_decay, callback is not None)
                     else:
-                        loss_value = self._lbfgs_step(lbfgs, avg_decay)
+                        step += 1
+                        self._iterate_lbfgs(lbfgs_state, step, avg_decay)
                     if callback is not None:
                         # host-side bookkeeping first: it overlaps the iteration still running on the device (the
                         # native path allocates nothing, so the high-water mark cannot move before the sync)
@@ -724,13 +726,12 @@ class StyleTransfer:
                         for device in self.devices:
                             if device.type == 'cuda':
                                 gpu_ram = max(gpu_ram, torch.cuda.max_memory_allocated(device))
-                        if optimizer == 'adam':
-                            if band is not None and self._comm_mode != 'peer':
-                                torch.cuda.current_stream().synchronize()   # host-driven exchanges: plain read-back
-                                self.last_loss_terms = self._loss_host.clone()
-                            else:   # the reference syncs here (loss.item()); this waits for the loss only
-                                self.last_loss_terms = self._wait_loss(step)
-                            loss_value = float(self.last_loss_terms[0])
+                        if band is not None and self._comm_mode != 'peer':
+                            torch.cuda.current_stream().synchronize()   # host-driven exchanges: plain read-back
+                            self.last_loss_terms = self._loss_host.clone()
+                        else:   # the reference syncs here (loss.item()); this waits for the loss only
+                            self.last_loss_terms = self._wait_loss(step)
+                        loss_value = float(self.last_loss_terms[0])
                         callback(STIterate(w=cw, h=ch, i=i, i_max=actual_its, loss=loss_value, time=time.time(),
                                            gpu_ram=gpu_ram))
 
@@ -748,20 +749,21 @@ class StyleTransfer:
 
         return self.get_image()
 
-    # ------------------------------------------------------------------ L-BFGS (ST:464-465): torch's optimizer on the
-    # host, closure evaluated by the native library
-    def _make_lbfgs(self):
-        self._lbfgs_param = torch.nn.Parameter(self.image, requires_grad=True)
-        return torch.optim.LBFGS([self._lbfgs_param], max_iter=1, history_size=10)
+    # ------------------------------------------------------------------ L-BFGS (ST:464-465): closure, torch's
+    # LBFGS.step (max_iter=1, history_size=10) and the EMA run natively as one CUDA graph per iteration (csrc/lbfgs.cu)
+    def _lbfgs_state(self, h, w):
+        """Fresh optimizer state for one scale (the reference builds a new optim.LBFGS per scale): a torch-owned block
+        of ~25 x 3HW floats (history ring, g, g_prev, d), so that max_memory_allocated stays truthful."""
+        lib = self.model.lib
+        n = ctypes.c_size_t()
+        _lib.check(lib.stb_lbfgs_state_bytes(h, w, ctypes.byref(n)))
+        state = torch.empty(n.value, dtype=torch.uint8, device=self._dev)
+        _lib.check(lib.stb_lbfgs_reset(_lib.ptr(state), h, w, _lib.cur_stream()))
+        return state
 
-    def _lbfgs_step(self, opt, avg_decay):
-        def closure():
-            terms, grad = self.loss_and_grad()
-            self._lbfgs_param.grad = grad
-            return terms[0].to(self._dev)
-
-        with torch.enable_grad():
-            loss = opt.step(closure)
-        self.average.value.mul_(avg_decay).add_(self.image, alpha=1 - avg_decay)
+    def _iterate_lbfgs(self, state, step, avg_decay):
+        """One L-BFGS iteration with no host sync; its loss is published to the loss ring under stamp `step`."""
+        m = self.model
+        _lib.check(m.lib.stb_iterate_lbfgs(m.ctx, _lib.ptr(self.image), _lib.ptr(self.average.value), _lib.ptr(state),
+                                           state.numel(), step, avg_decay, None, _lib.cur_stream()))
         self.average.note_update()
-        return float(loss)
