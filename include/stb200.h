@@ -96,7 +96,7 @@ STB_API int stb_iterate_ex(stb_ctx* ctx, float* img, float* exp_avg, float* exp_
  * The optimizer state (history ring, g, g_prev, d, scalars) is ONE caller-owned device block of
  * stb_lbfgs_state_bytes(H, W) bytes, 256-byte aligned (~25 x 3HW floats: ~1.26 GB at 2048^2).  The reference builds
  * a fresh optim.LBFGS per scale: call stb_lbfgs_reset once per scale, before its first iteration.
- * stb_iterate_lbfgs runs on the targets' H x W (stb_set_targets) and needs a context without a band.  It is one
+ * stb_iterate_lbfgs runs on the targets' H x W (stb_set_targets) and needs a context without a band (stb_iterate_lbfgs_banded runs a band).  It is one
  * stream-ordered sequence, replayed as a CUDA graph, with no host sync; the loss of the PRE-step image goes to the loss
  * ring (stb_set_loss_ring) under the stamp `step`, the running iteration count of the whole stylize() call, and
  * optionally to loss_out_host8. */
@@ -172,6 +172,15 @@ STB_API int stb_comm_reset(stb_ctx* ctx, void* stream);
 STB_API int stb_iterate_banded(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step,
                                float lr, float beta1, float beta2, float adam_eps, float ema_decay,
                                float* loss_out_host8, void* stream);
+/* optimizer='lbfgs' on a band: the iteration of stb_iterate_banded up to the seam, then the L-BFGS step of
+ * stb_iterate_lbfgs on this band's own rows.  The state holds the own rows only: stb_lbfgs_state_bytes(own_rows, W)
+ * bytes, reset once per scale with stb_lbfgs_reset.  Every dot product of the step is summed over the ranks inside the
+ * graph (a one-block kernel per reduction, ranks combined in rank order), so every rank holds bit-identical scalars
+ * and takes the same branches.  img / ema: the local [1,3,h_local,W] band; only the own rows are updated, the halo rows
+ * are refreshed from the neighbours.  STB_ERR_STATE without a band, a comm connection and geometry, or when the
+ * geometry does not match the band; STB_ERR_INVALID for a state that is too small or misaligned. */
+STB_API int stb_iterate_lbfgs_banded(stb_ctx* ctx, float* img, float* ema, void* state, size_t state_bytes,
+                                     int64_t step, float ema_decay, float* loss_out_host8, void* stream);
 /* 1: iterations replay as CUDA graphs, 2: enabled but nothing captured yet, 0: eager launches (note_out says why). */
 STB_API int stb_graph_status(stb_ctx* ctx, char* note_out, size_t note_bytes);
 /* Kernel launches issued through graph replays so far, counted from the captured graphs: number of replays, kernels

@@ -43,6 +43,17 @@ STB_API size_t stb_test_w2_workspace_bytes(void);
  * call then synchronises the stream): history pairs held and step length of the current direction. */
 STB_API int stb_test_lbfgs_step(void* state, size_t bytes, int H, int W, float* x, const float* grad, float* ema,
                                 float ema_decay, int* pairs_out, float* t_out, void* stream);
+/* load every kernel of the test library now (lazy module loading would otherwise synchronise the context at a first
+ * launch, which deadlocks against a peer's resident wait kernel): call once before ranks step concurrently */
+STB_API int stb_test_preload(void);
+/* the banded L-BFGS step of stb_iterate_lbfgs_banded alone, on a context whose comm connection and geometry are set
+ * (stb_comm_connect_*, stb_comm_set_geometry): comm phase 0, halo pull into x, grad (this rank's local gradient,
+ * [3][h_local][W]) into the mailbox, phase 2, the banded step (seam gather with the neighbours' apron rows when
+ * add_seams, cross-rank reductions, own-row update of x / ema [3][h_local][W], outbox fill) and phase 3.  The state
+ * has stb_lbfgs_state_bytes(own_rows, W) bytes.  pairs_out / t_out as for stb_test_lbfgs_step. */
+STB_API int stb_test_lbfgs_step_banded(stb_ctx* ctx, void* state, size_t bytes, float* x, const float* grad,
+                                       float* ema, float ema_decay, int add_seams, int* pairs_out, float* t_out,
+                                       void* stream);
 
 #ifdef __cplusplus
 }

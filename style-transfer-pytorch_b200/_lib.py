@@ -65,6 +65,7 @@ def _declare(lib):
         'stb_comm_set_geometry': [vp, i, i, i, i, i, i, i, i],
         'stb_comm_reset': [vp, vp],
         'stb_iterate_banded': [vp, vp, vp, vp, vp, i64, f, f, f, f, f, vp, vp],
+        'stb_iterate_lbfgs_banded': [vp, vp, vp, vp, sz, i64, f, vp, vp],
         'stb_graph_status': [vp, C.c_char_p, sz],
         'stb_launch_count': [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i)],
         'stb_profile_enable': [vp, i],
@@ -90,7 +91,10 @@ def _declare_test(lib):
         'stb_test_gram': [vp, C.c_long, i, vp, sz, vp, vp, vp],
         'stb_test_w2': [vp, vp, vp, vp, i, f, f, vp, sz, vp, vp, vp, vp, vp],
         'stb_test_lbfgs_step': [vp, sz, i, i, vp, vp, vp, f, C.POINTER(i), C.POINTER(f), vp],
+        'stb_test_lbfgs_step_banded': [vp, vp, sz, vp, vp, vp, f, i, C.POINTER(i), C.POINTER(f), vp],
     })
+    lib.stb_test_preload.argtypes = []
+    lib.stb_test_preload.restype = C.c_int
     lib.stb_test_gram_partials_floats.argtypes = [C.c_long, i]
     lib.stb_test_gram_partials_floats.restype = sz
     lib.stb_test_w2_workspace_bytes.argtypes = []
@@ -106,13 +110,14 @@ EXPORTS = [
     'stb_set_loss_ring', 'stb_resize', 'stb_comm_create', 'stb_comm_connect_ipc', 'stb_comm_connect_local', 'stb_comm_disconnect', 'stb_comm_alloc_workspace',
     'stb_comm_connect_ws_ipc', 'stb_comm_connect_ws_local', 'stb_comm_release_workspace',
     'stb_comm_set_geometry', 'stb_comm_reset',
-    'stb_iterate_banded', 'stb_graph_status', 'stb_launch_count', 'stb_profile_enable', 'stb_profile_read', 'stb_debug_activation', 'stb_debug_w2_trace',
+    'stb_iterate_banded', 'stb_iterate_lbfgs_banded', 'stb_graph_status', 'stb_launch_count', 'stb_profile_enable', 'stb_profile_read', 'stb_debug_activation', 'stb_debug_w2_trace',
 ]
 # include/stb200_test.h (libstb200_test.so)
 TEST_EXPORTS = [
     'stb_test_last_error', 'stb_pack_weights', 'stb_test_pixel_gemm', 'stb_test_conv0_fwd', 'stb_test_conv0_bwd',
     'stb_test_conv_pool', 'stb_test_pool_bwd', 'stb_test_gram', 'stb_test_gram_partials_floats', 'stb_test_w2',
-    'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step',
+    'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step', 'stb_test_lbfgs_step_banded',
+    'stb_test_preload',
 ]
 
 

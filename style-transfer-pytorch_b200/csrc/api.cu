@@ -114,8 +114,8 @@ struct stb_ctx {
     }
   };
   // 0: stb_iterate, 1: stb_iterate_fwd, 2: stb_iterate_bwd (host-driven phases), 3: stb_iterate_banded,
-  // 4: stb_iterate_lbfgs
-  GraphSlot gslot[5];
+  // 4: stb_iterate_lbfgs, 5: stb_iterate_lbfgs_banded
+  GraphSlot gslot[6];
   void reset_graphs() { for (auto& g : gslot) g.reset(); }
   bool graphs_enabled = true;
   std::string graph_note;  // why graph replay was switched off for this context (stb_graph_status)
@@ -815,6 +815,11 @@ int run_graphed(stb_ctx* ctx, int slot, const stb_ctx::GraphKey& key, bool allow
   return STB_OK;
 }
 
+namespace stb {
+// the test library's banded L-BFGS hook (api_test.cu) runs on a context's comm connection and geometry
+const CommDev* ctx_comm(const stb_ctx* ctx) { return ctx->comm_ready && ctx->comm_geometry ? &ctx->comm : nullptr; }
+}  // namespace stb
+
 extern "C" {
 
 // One pass of ST:480-486.  apply_update = 0 evaluates loss / gradient only (test hook, L-BFGS closure).
@@ -1058,6 +1063,7 @@ int stb_comm_create(stb_ctx* ctx, int rank, int world, int max_h_local, int max_
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(reduce2_kernel)));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(adam_scalars_kernel)));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(finalize_loss_kernel)));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(advance_step_kernel)));
   return STB_OK;
 }
 
@@ -1280,6 +1286,65 @@ int stb_iterate_banded(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_
   key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = exp_avg; key.v = exp_avg_sq; key.ema = ema;
   key.loss = loss_out_host8; key.lr = lr; key.b1 = beta1; key.b2 = beta2; key.eps = adam_eps; key.decay = ema_decay;
   return run_graphed(ctx, 3, key, true, s, run);
+}
+
+// optimizer='lbfgs' on a band: the sequence of stb_iterate_banded up to the gradient stamp, then the banded L-BFGS step
+// of lbfgs.cu (seam gather, cross-rank reductions, own-row update + outbox fill) and the halo stamp.  The state holds
+// this band's own rows only: stb_lbfgs_state_bytes(own_rows, W).
+int stb_iterate_lbfgs_banded(stb_ctx* ctx, float* img, float* ema, void* state, size_t state_bytes, int64_t step,
+                             float ema_decay, float* loss_out_host8, void* stream) {
+  STB_CHECK(ctx && img && ema && state, STB_ERR_INVALID, "null argument");
+  STB_ENTER(ctx);
+  STB_CHECK(ctx->targets_set && ctx->band_on, STB_ERR_STATE, "stb_set_band + stb_set_targets must precede");
+  STB_CHECK(ctx->comm_ready && ctx->comm_geometry, STB_ERR_STATE, "stb_comm_connect_* + stb_comm_set_geometry first");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  Plan pl;
+  make_plan(ctx, ctx->tH, ctx->tW, &pl);
+  STB_TRY(ensure_ws(ctx, pl));
+  const CommDev& c = ctx->comm;
+  STB_CHECK(c.h_local == pl.H && c.W == pl.W && c.own0 == ctx->band_own0 && c.own_rows == ctx->band_own_rows,
+            STB_ERR_STATE, "comm geometry (%dx%d, own %d+%d) does not match the band (%dx%d, own %d+%d)", c.h_local,
+            c.W, c.own0, c.own_rows, pl.H, pl.W, ctx->band_own0, ctx->band_own_rows);
+  STB_CHECK(step >= 1, STB_ERR_INVALID, "step must be >= 1");
+  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(ema) & 15) == 0,
+            STB_ERR_INVALID, "state must be 256-byte aligned, img and ema 16-byte aligned");
+  const long n = 3l * c.own_rows * c.W;
+  STB_CHECK(state_bytes >= lbfgs_state_bytes(n), STB_ERR_INVALID,
+            "L-BFGS state of %zu bytes is too small for %d own rows x %d (needs %zu)", state_bytes, c.own_rows, c.W,
+            lbfgs_state_bytes(n));
+  if (ctx->dev_step_mirror != step - 1) {
+    const long long v = step - 1;
+    STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &v, sizeof(v), cudaMemcpyHostToDevice, s));
+    STB_CUDA_CHECK(cudaStreamSynchronize(s));  // `v` is a stack variable; this path runs once per scale at most
+  }
+  ctx->dev_step_mirror = step;
+  float* grad = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_grad);
+  HaloPlans hp;
+  const HaloPlans* halo = nullptr;
+  if (ctx->halo_mode) {
+    STB_CHECK(ctx->ws == ctx->shared_ws && ctx->shared_ws != nullptr, STB_ERR_STATE,
+              "halo mode needs the library-owned workspace bound (stb_comm_alloc_workspace)");
+    make_plan(ctx, c.rank > 0 ? c.up_h_local : pl.H, pl.W, &hp.up);
+    make_plan(ctx, c.rank + 1 < c.world ? c.dn_h_local : pl.H, pl.W, &hp.dn);
+    halo = &hp;
+  }
+  auto run = [&]() -> int {
+    ctx->halo_seq = 0;
+    STB_TRY(launch_comm_phase(c, 0, s));
+    STB_TRY(launch_halo_pull(c, img, s));
+    STB_TRY(iterate_fwd(ctx, pl, img, s, halo));
+    STB_TRY(launch_stats_allreduce(c, at<float>(ctx, pl.stats_off), pl.stats_floats, s));
+    advance_step_kernel<<<1, 1, 0, s>>>(ctx->d_step);
+    STB_TRY(iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad, loss_out_host8, s, halo));
+    STB_TRY(launch_comm_phase(c, 2, s));
+    STB_TRY(launch_lbfgs_step_banded(state, c, img, ema, ema_decay, halo ? 0 : 1, s));
+    return launch_comm_phase(c, 3, s);
+  };
+  stb_ctx::GraphKey key{};
+  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = state; key.ema = ema;
+  key.loss = loss_out_host8; key.decay = ema_decay;
+  return run_graphed(ctx, 5, key, true, s, run);
 }
 
 // Sync-free loss read-back (SURVEY.md 8f row 2).  host_ring: PINNED host memory of slots x 16 floats (NULL: off).

@@ -117,6 +117,38 @@ int stb_test_lbfgs_step(void* state, size_t bytes, int H, int W, float* x, const
   return STB_OK;
 }
 
+// Loads every kernel of THIS library (it holds its own copies of the product kernels).  A banded test step must not be
+// the first launch of a kernel: a lazy module load synchronises the context, which deadlocks against a peer's resident
+// wait kernel (see comm_preload).
+int stb_test_preload(void) {
+  STB_TRY(comm_preload()); STB_TRY(preload_conv_kernels()); STB_TRY(preload_gram_kernels());
+  STB_TRY(preload_w2_kernels()); STB_TRY(preload_conv0_kernels()); STB_TRY(preload_image_kernels());
+  return STB_OK;
+}
+
+// The banded step of stb_iterate_lbfgs_banded on a scripted gradient, on a context with a comm connection and geometry:
+// comm phase 0, halo pull, grad [3][h_local][W] into the mailbox, phase 2, the banded step, phase 3.
+int stb_test_lbfgs_step_banded(stb_ctx* ctx, void* state, size_t bytes, float* x, const float* grad, float* ema,
+                               float ema_decay, int add_seams, int* pairs_out, float* t_out, void* stream) {
+  STB_CHECK(ctx && state && x && grad && ema, STB_ERR_INVALID, "null argument");
+  const CommDev* c = ctx_comm(ctx);
+  STB_CHECK(c != nullptr, STB_ERR_STATE, "stb_comm_connect_* + stb_comm_set_geometry first");
+  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(ema) & 15) == 0,
+            STB_ERR_INVALID, "state must be 256-byte aligned, x and ema 16-byte aligned");
+  STB_CHECK(bytes >= lbfgs_state_bytes(3l * c->own_rows * c->W), STB_ERR_INVALID, "L-BFGS state too small");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  STB_TRY(launch_comm_phase(*c, 0, s));
+  STB_TRY(launch_halo_pull(*c, x, s));
+  STB_CUDA_CHECK(cudaMemcpyAsync(c->mbox[c->rank] + c->off_grad, grad, 3ul * c->h_local * c->W * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, s));
+  STB_TRY(launch_comm_phase(*c, 2, s));
+  STB_TRY(launch_lbfgs_step_banded(state, *c, x, ema, ema_decay, add_seams, s));
+  STB_TRY(launch_comm_phase(*c, 3, s));
+  if (pairs_out || t_out) STB_TRY(lbfgs_read_info(state, pairs_out, t_out, s));
+  return STB_OK;
+}
+
 size_t stb_test_w2_workspace_bytes(void) { return W2Engine::workspace_bytes(); }
 
 // Runs the W2 engine with the given problem placed in the slot of matching size (other slots get a benign

@@ -20,9 +20,11 @@
 //                       deterministic, and bit-identical on every rank, so the replicated W2 chain stays in lock step
 //   adam_seam_kernel    seam reduce of the image gradient (own + neighbours' apron rows) fused with Adam + clamp + EMA
 //                       (torch/optim/adam.py:413-546, ST:483-486) and with the fill of the outboxes
+//   lbfgs_seam_gather   the same seam reduce for the banded L-BFGS step (lbfgs.cu), into its compact gradient
 // A wait that is not satisfied within CommDev::timeout_ns (30 s; STB_COMM_TIMEOUT_S) traps (the launch fails with a CUDA error) instead of hanging.
 #include <cstring>
 
+#include "comm.cuh"
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -30,45 +32,15 @@ namespace stb {
 
 namespace {
 
-__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
-  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
 // Row-wise kernels run on float4 when the image width is a multiple of 4 (rows are then 16-byte aligned) and on
 // scalars otherwise (odd pyramid widths such as 181 or 543).
 template <int V> struct Vec;
 template <> struct Vec<4> { typedef float4 T; };
 template <> struct Vec<1> { typedef float T; };
-// peer data: the local L1 may hold a stale copy of a remote line (peer accesses bypass the local L2 but not L1)
-__device__ __forceinline__ float4 ld_peer(const float4* p) { return __ldcv(p); }
-__device__ __forceinline__ float ld_peer(const float* p) { return __ldcv(p); }
 __device__ __forceinline__ void unpack(const float4& v, float (&a)[4]) { a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w; }
 __device__ __forceinline__ void unpack(const float& v, float (&a)[1]) { a[0] = v; }
 __device__ __forceinline__ void pack(float4& v, const float (&a)[4]) { v = make_float4(a[0], a[1], a[2], a[3]); }
 __device__ __forceinline__ void pack(float& v, const float (&a)[1]) { v = a[0]; }
-
-__device__ void wait_stamp(const unsigned long long* flag, unsigned long long want, unsigned long long* err,
-                           unsigned long long timeout_ns) {
-  if (ld_acquire_sys(flag) >= want) return;
-  const unsigned long long t0 = globaltimer_ns();
-  unsigned spins = 0;
-  while (ld_acquire_sys(flag) < want) {
-    if ((++spins & 0xFF) == 0 && globaltimer_ns() - t0 > timeout_ns) {
-      *err = want;
-      __threadfence_system();
-      __trap();
-    }
-  }
-}
 
 // phase 0 BEGIN : t = ++iter;                     wait halo  stamps of the neighbours >= t - 1
 // phase 1 STATS : publish stats stamp = t;        wait stats stamps of ALL ranks      >= t
@@ -244,6 +216,37 @@ adam_seam_kernel(CommDev c, float* __restrict__ img, float* __restrict__ exp_avg
   }
 }
 
+// banded L-BFGS: g[3][own_rows][W] (compact) = the own rows of the local gradient (+ the neighbours' apron rows), summed
+// in the order of adam_seam_kernel: own, upper, lower
+template <int V>
+__global__ void __launch_bounds__(256) lbfgs_seam_gather_kernel(CommDev c, float* __restrict__ g, int add_seams) {
+  typedef typename Vec<V>::T T;
+  const int w4 = c.W / V;
+  const long per = (long)c.own_rows * w4;
+  const T* grad = reinterpret_cast<const T*>(c.mbox[c.rank] + c.off_grad);
+  const bool has_up = c.rank > 0 && add_seams, has_dn = c.rank + 1 < c.world && add_seams;
+  const T* gup = has_up ? reinterpret_cast<const T*>(c.mbox[c.rank - 1] + c.off_grad) : nullptr;
+  const T* gdn = has_dn ? reinterpret_cast<const T*>(c.mbox[c.rank + 1] + c.off_grad) : nullptr;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < 3 * per; i += (long)gridDim.x * blockDim.x) {
+    const int ch = (int)(i / per);
+    const long r4 = i - (long)ch * per;
+    const int r = (int)(r4 / w4), x4 = (int)(r4 - (long)r * w4);
+    float gg[V], aa[V];
+    unpack(grad[((long)ch * c.h_local + c.own0 + r) * w4 + x4], gg);
+    if (has_up && r < COMM_APRON) {
+      unpack(ld_peer(gup + ((long)ch * c.up_h_local + c.up_apron_row0 + r) * w4 + x4), aa);
+#pragma unroll
+      for (int k = 0; k < V; ++k) gg[k] += aa[k];
+    }
+    if (has_dn && r >= c.own_rows - COMM_APRON) {
+      unpack(ld_peer(gdn + ((long)ch * c.dn_h_local + (r - (c.own_rows - COMM_APRON))) * w4 + x4), aa);
+#pragma unroll
+      for (int k = 0; k < V; ++k) gg[k] += aa[k];
+    }
+    pack(reinterpret_cast<T*>(g)[i], gg);
+  }
+}
+
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 int grid_for(long n) {
@@ -275,7 +278,9 @@ int comm_preload() {
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, adam_seam_kernel<4>));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, adam_seam_kernel<1>));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, halo_rows_kernel));
-  return STB_OK;
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_seam_gather_kernel<4>));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_seam_gather_kernel<1>));
+  return preload_lbfgs_kernels();
 }
 
 int launch_comm_phase(const CommDev& c, int phase, cudaStream_t s) {
@@ -328,6 +333,15 @@ int launch_adam_seam(const CommDev& c, float* img, float* exp_avg, float* exp_av
   else
     adam_seam_kernel<1><<<grid_for(3l * c.own_rows * c.W), 256, 0, s>>>(c, img, exp_avg, exp_avg_sq, ema, d_adam,
                                                                         add_seams);
+  STB_CUDA_CHECK(cudaGetLastError());
+  return STB_OK;
+}
+
+int launch_lbfgs_seam_gather(const CommDev& c, float* g, int add_seams, cudaStream_t s) {
+  if (c.W % 4 == 0)
+    lbfgs_seam_gather_kernel<4><<<grid_for(3l * c.own_rows * (c.W / 4)), 256, 0, s>>>(c, g, add_seams);
+  else
+    lbfgs_seam_gather_kernel<1><<<grid_for(3l * c.own_rows * c.W), 256, 0, s>>>(c, g, add_seams);
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
 }

@@ -84,6 +84,16 @@ int launch_lbfgs_reset(void* state, cudaStream_t s);
 int launch_lbfgs_step(void* state, long n, float* x, float* ema, float ema_decay, cudaStream_t s);
 // synchronous read of the pair count and the step length t of the current direction (test hook)
 int lbfgs_read_info(const void* state, int* pairs, float* t, cudaStream_t s);
+struct CommDev;
+// Banded step of a tiled iteration (a rank's own rows only; the state holds n = 3 * own_rows * W floats).  Runs after
+// comm phase 2, with this rank's local gradient [3][h_local][W] in its mailbox: seam gather into the compact g, then the
+// launch sequence of launch_lbfgs_step with a one-block cross-rank reduction (lbfgs_xreduce_kernel) after pass 0 and
+// after every round, so that every rank holds the same global scalars; the final pass updates the own rows of the local
+// image x / ema [3][h_local][W] and fills the outboxes.
+constexpr int LBFGS_XREDUCES = 2 * STB_LBFGS_HISTORY + 2;   // pass 0 + 21 rounds
+int launch_lbfgs_step_banded(void* state, const CommDev& c, float* x, float* ema, float ema_decay, int add_seams,
+                             cudaStream_t s);
+int preload_lbfgs_kernels();
 
 // ---------------------------------------------------------------- Gram / channel sums on wgmma (gram_tc.cu)
 int gram_num_splits(long P, int C);
@@ -154,8 +164,10 @@ struct W2Engine {
 // ---------------------------------------------------------------- multi-GPU peer-memory exchange (comm.cu)
 constexpr int COMM_APRON = 80;       // halo rows on each interior side of a band (receptive-field radius of relu5_1)
 constexpr int COMM_MAX_RANKS = 8;
-// u64 slots at the head of a mailbox (one 128-byte line each)
-enum { COMM_ITER = 0, COMM_FLAG_STATS = 16, COMM_FLAG_GRAD = 32, COMM_FLAG_HALO = 48, COMM_ERR = 64, COMM_PROG = 80 };
+// u64 slots at the head of a mailbox (one 128-byte line each; the head is 4096 bytes, zeroed by stb_comm_reset).
+// COMM_XVAL: the banded L-BFGS step's cross-rank reductions, [2 (iteration parity)][LBFGS_XREDUCES][4] doubles.
+enum { COMM_ITER = 0, COMM_FLAG_STATS = 16, COMM_FLAG_GRAD = 32, COMM_FLAG_HALO = 48, COMM_ERR = 64, COMM_PROG = 80,
+       COMM_FLAG_XRED = 96, COMM_XVAL = 112 };
 struct CommDev {  // passed by value to the exchange kernels
   int rank, world;
   uint8_t* mbox[COMM_MAX_RANKS];   // mailbox of every rank as mapped into THIS process (own one included)
@@ -174,6 +186,8 @@ int launch_halo_pull(const CommDev& c, float* img, cudaStream_t s);
 int launch_stats_allreduce(const CommDev& c, float* stats, size_t n_floats, cudaStream_t s);
 int launch_adam_seam(const CommDev& c, float* img, float* exp_avg, float* exp_avg_sq, float* ema,
                      const AdamScalars* d_adam, int add_seams, cudaStream_t s);
+// g[3][own_rows][W] = own rows of the mailbox gradient (+ the neighbours' apron rows when add_seams)
+int launch_lbfgs_seam_gather(const CommDev& c, float* g, int add_seams, cudaStream_t s);
 // per-layer halo exchange: publish progress stamp `seq` of this iteration, wait for the neighbours' same stamp, then copy
 // one boundary row (row_bytes) from each neighbour's buffer into this rank's halo rows.  Pointers are absolute (peer
 // workspaces are mapped); a null source / destination skips that side.
@@ -186,6 +200,9 @@ struct HaloRowArgs {
   int seq;
 };
 int launch_halo_rows(const CommDev& c, const HaloRowArgs& a, cudaStream_t s);
+
+// the comm connection of a context when it is connected and has a geometry, else null (test hooks)
+const CommDev* ctx_comm(const stb_ctx* ctx);
 
 // force every kernel of the library into the context (lazy module loading may otherwise synchronise the context at
 // a first launch, which deadlocks against a resident peer-wait kernel)

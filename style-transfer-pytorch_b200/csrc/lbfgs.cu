@@ -15,11 +15,15 @@
 //                   2 * count + 1 operations runs in the LAST rounds, earlier rounds return at once, so the final pass
 //                   always finds g.d in the same partial buffer.
 //   final           g.d test, x += t * d, EMA, g_prev = g
+// The banded step of a tiled iteration (launch_lbfgs_step_banded) runs the same kernels on a rank's own rows, with a
+// one-block cross-rank reduction (lbfgs_xreduce_kernel) after pass 0 and after every round: the consumers then read one
+// partial, the global value, which every rank summed in rank order and therefore holds bit for bit.
 // Dot products are reduced deterministically: fixed grid for a given n, one fp64 partial per block, and every block
 // of the consuming kernel sums the partials in the same fixed order (graph replay == eager, bit for bit).  Scalars
 // are rounded to fp32 where torch holds fp32 tensors (ys, ro, H_diag, al, be, t, gtd and the comparisons).
 #include <type_traits>
 
+#include "comm.cuh"
 #include "kernels.h"
 
 namespace stb {
@@ -230,7 +234,7 @@ __global__ void __launch_bounds__(LB_THREADS) lbfgs_decide_kernel(LbState s, int
   }
 }
 
-// round r of the two-loop recursion.  With c pairs the active operations o = 0 .. 2c run in rounds
+// round r of the two-loop recursion (the previous round left np partials).  With c pairs the active operations o = 0 .. 2c run in rounds
 // r = LB_ROUNDS - (2c + 1) + o:
 //   o = 0        v = -g                          (torch: q = -g)
 //   1 <= o <= c  v -= al_i y_i, i = c - o        (al_i = (s_i . q) ro_i, the dot of the previous round)
@@ -238,7 +242,7 @@ __global__ void __launch_bounds__(LB_THREADS) lbfgs_decide_kernel(LbState s, int
 //   o > c        v += (al_i - be_i) s_i, i = o-c-1 (be_i = (y_i . r) ro_i)
 // v is stored into d (q and r share it, as in torch) and the dot the next operation needs is accumulated:
 // s_{c-1-o} . v while o < c, y_{o-c} . v while o < 2c, and g . d (gtd) at o = 2c.
-__global__ void __launch_bounds__(LB_THREADS) lbfgs_round_kernel(LbState s, int round) {
+__global__ void __launch_bounds__(LB_THREADS) lbfgs_round_kernel(LbState s, int round, int np) {
   __shared__ double sm[33];
   const LbHeader& h = *s.hdr;
   if (h.skip) return;
@@ -248,7 +252,7 @@ __global__ void __launch_bounds__(LB_THREADS) lbfgs_round_kernel(LbState s, int 
   float coef = 0.f;
   const float* upd = nullptr;
   if (o >= 1) {
-    const float dot = (float)reduce_partials(s.part + ((round - 1) & 1) * LB_MAX_BLOCKS, gridDim.x, sm);
+    const float dot = (float)reduce_partials(s.part + ((round - 1) & 1) * LB_MAX_BLOCKS, np, sm);
     if (o <= c) {
       const int slot = ring_slot(h, c - o);
       const float al = dot * h.ro[slot];
@@ -289,34 +293,128 @@ __global__ void __launch_bounds__(LB_THREADS) lbfgs_round_kernel(LbState s, int 
   if (threadIdx.x == 0) s.part[(round & 1) * LB_MAX_BLOCKS + blockIdx.x] = acc;
 }
 
+// g.d test of the final pass over the np partials of the last round: whether x moves (false on an opt_cond step)
+__device__ __forceinline__ bool final_take(const LbState& s, int np, double* sm) {
+  if (s.hdr->skip) return false;
+  const float gtd = (float)reduce_partials(s.part + ((LB_ROUNDS - 1) & 1) * LB_MAX_BLOCKS, np, sm);
+  const bool take = !(gtd > -1e-9f);
+  if (blockIdx.x == 0 && threadIdx.x == 0) { s.hdr->gtd = gtd; s.hdr->took_step = take; }
+  return take;
+}
+
+// the per-element work of the final pass, shared by the untiled and the banded kernel: x += t d (no clamp) when the
+// step is taken, EMA of x, g_prev = g.  x / ema at jx, the state vectors at j; xv receives the new x.
+template <int L>
+__device__ __forceinline__ void final_elems(const LbState& s, bool take, bool skip, float t, float decay, float* x,
+                                            float* ema, long jx, long j, Vec<L>& xv) {
+  const float om = 1.f - decay;
+  xv = ld<L>(x, jx);
+  if (take) {
+    const Vec<L> d = ld<L>(s.d, j);
+#pragma unroll
+    for (int k = 0; k < L; ++k) xv.v[k] = xv.v[k] + t * d.v[k];
+    st<L>(x, jx, xv);
+  }
+  Vec<L> e = ld<L>(ema, jx);
+#pragma unroll
+  for (int k = 0; k < L; ++k) e.v[k] = e.v[k] * decay + om * xv.v[k];
+  st<L>(ema, jx, e);
+  if (!skip) st<L>(s.g_prev, j, ld<L>(s.g, j));
+}
+
 // final pass: g.d test, x += t d (no clamp), EMA of x, g_prev = g
 __global__ void __launch_bounds__(LB_THREADS) lbfgs_final_kernel(LbState s, float* __restrict__ x,
-                                                                 float* __restrict__ ema, float decay) {
+                                                                 float* __restrict__ ema, float decay, int np) {
   __shared__ double sm[33];
-  const LbHeader& h = *s.hdr;
-  const bool skip = h.skip != 0;
-  bool take = false;
-  if (!skip) {
-    const float gtd = (float)reduce_partials(s.part + ((LB_ROUNDS - 1) & 1) * LB_MAX_BLOCKS, gridDim.x, sm);
-    take = !(gtd > -1e-9f);
-    if (blockIdx.x == 0 && threadIdx.x == 0) { s.hdr->gtd = gtd; s.hdr->took_step = take; }
-  }
-  const float t = h.t, om = 1.f - decay;
+  const bool skip = s.hdr->skip != 0;
+  const bool take = final_take(s, np, sm);
+  const float t = s.hdr->t;
   for_each(s.n, [&](auto lanes, long j) {
     constexpr int L = decltype(lanes)::value;
-    Vec<L> xv = ld<L>(x, j);
-    if (take) {
-      const Vec<L> d = ld<L>(s.d, j);
-#pragma unroll
-      for (int k = 0; k < L; ++k) xv.v[k] = xv.v[k] + t * d.v[k];
-      st<L>(x, j, xv);
-    }
-    Vec<L> e = ld<L>(ema, j);
-#pragma unroll
-    for (int k = 0; k < L; ++k) e.v[k] = e.v[k] * decay + om * xv.v[k];
-    st<L>(ema, j, e);
-    if (!skip) st<L>(s.g_prev, j, ld<L>(s.g, j));
+    Vec<L> xv;
+    final_elems<L>(s, take, skip, t, decay, x, ema, j, j, xv);
   });
+}
+
+// ---- banded step (tiled iteration): the state vectors are compact [3][own_rows][W]; x and ema are the local
+// [3][h_local][W] image.  V = 4 when W % 4 == 0 (rows are 16-byte aligned), else 1 (odd pyramid widths such as 181).
+
+// Cross-rank reduction, one block.  nvals (<= 4) values; value k has nb block partials at part + k * LB_MAX_BLOCKS
+// (value 0 is a NaN-propagating max when max0).  This rank's sums, taken in reduce_partials' order, go to its mailbox
+// slot [iteration parity][seq] and are published by the stamp iter * 32 + seq (system-scope release).  Lane r of warp 0
+// waits for rank r's stamp (acquire, wait_stamp's timeout) and loads rank r's values; thread 0 combines the ranks in
+// rank order -- the same order on every rank, so every rank gets the same bits -- and stores the global values at
+// part[k * LB_MAX_BLOCKS], where the next kernel reads them as its only partial.  Peer waits happen here and never in
+// the full-grid kernels: ranks that share a GPU must not hold its SMs while they wait.
+__global__ void __launch_bounds__(LB_THREADS) lbfgs_xreduce_kernel(CommDev c, double* part, int nvals, int nb,
+                                                                   int max0, int seq) {
+  __shared__ double sm[33];
+  __shared__ double vals[COMM_MAX_RANKS][4];
+  double mine[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (k < nvals)
+      mine[k] = k == 0 && max0 ? reduce_partials<true>(part + k * LB_MAX_BLOCKS, nb, sm)
+                               : reduce_partials(part + k * LB_MAX_BLOCKS, nb, sm);
+  unsigned long long* own = reinterpret_cast<unsigned long long*>(c.mbox[c.rank]);
+  const unsigned long long it = own[COMM_ITER];
+  const int slot = COMM_XVAL + ((int)(it & 1) * LBFGS_XREDUCES + seq) * 4;
+  const unsigned long long want = it * 32ull + (unsigned long long)seq;
+  if (threadIdx.x == 0) {
+    double* mv = reinterpret_cast<double*>(own + slot);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < nvals) { mv[k] = mine[k]; vals[c.rank][k] = mine[k]; }
+    __threadfence_system();
+    st_release_sys(own + COMM_FLAG_XRED, want);
+  }
+  const int lane = threadIdx.x;
+  if (lane < c.world && lane != c.rank) {
+    const unsigned long long* peer = reinterpret_cast<const unsigned long long*>(c.mbox[lane]);
+    wait_stamp(peer + COMM_FLAG_XRED, want, own + COMM_ERR, c.timeout_ns);
+    const double* pv = reinterpret_cast<const double*>(peer + slot);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < nvals) vals[lane][k] = ld_peer(pv + k);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < nvals) {
+        double v = vals[0][k];
+        for (int r = 1; r < c.world; ++r) v = k == 0 && max0 ? nan_max(v, vals[r][k]) : v + vals[r][k];
+        part[k * LB_MAX_BLOCKS] = v;
+      }
+  }
+}
+static_assert(COMM_XVAL + 2 * LBFGS_XREDUCES * 4 <= 4096 / 8, "cross-rank values must fit the mailbox head");
+static_assert(LBFGS_XREDUCES < 32, "stamp = iteration * 32 + seq");
+
+// final pass of the banded step on the own rows of the local image; the first / last COMM_APRON rows also go to the
+// outboxes (the neighbours' next halo), as adam_seam_kernel does
+template <int V>
+__global__ void __launch_bounds__(LB_THREADS) lbfgs_final_banded_kernel(LbState s, CommDev c, float* __restrict__ x,
+                                                                        float* __restrict__ ema, float decay) {
+  __shared__ double sm[33];
+  const bool skip = s.hdr->skip != 0;
+  const bool take = final_take(s, 1, sm);
+  const float t = s.hdr->t;
+  const int wv = c.W / V;
+  const int per = c.own_rows * wv;   // 3 * per < 2^31 (launch_lbfgs_step_banded)
+  float* out_first = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_outbox[0]);
+  float* out_last = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_outbox[1]);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * per; i += gridDim.x * blockDim.x) {
+    const int ch = i / per;
+    const int r4 = i - ch * per;
+    const int r = r4 / wv;
+    const long xo = (long)(r4 - r * wv) * V;
+    Vec<V> xv;
+    final_elems<V>(s, take, skip, t, decay, x, ema, ((long)ch * c.h_local + c.own0 + r) * c.W + xo, (long)i * V, xv);
+    if (r < COMM_APRON) st<V>(out_first, ((long)ch * COMM_APRON + r) * c.W + xo, xv);
+    if (r >= c.own_rows - COMM_APRON)
+      st<V>(out_last, ((long)ch * COMM_APRON + (r - (c.own_rows - COMM_APRON))) * c.W + xo, xv);
+  }
 }
 
 }  // namespace
@@ -337,9 +435,40 @@ int launch_lbfgs_step(void* state, long n, float* x, float* ema, float ema_decay
   const int nb = lb_blocks(n);
   lbfgs_pass0_kernel<<<nb, LB_THREADS, 0, s>>>(st);
   lbfgs_decide_kernel<<<1, LB_THREADS, 0, s>>>(st, nb);
-  for (int r = 0; r < LB_ROUNDS; ++r) lbfgs_round_kernel<<<nb, LB_THREADS, 0, s>>>(st, r);
-  lbfgs_final_kernel<<<nb, LB_THREADS, 0, s>>>(st, x, ema, ema_decay);
+  for (int r = 0; r < LB_ROUNDS; ++r) lbfgs_round_kernel<<<nb, LB_THREADS, 0, s>>>(st, r, nb);
+  lbfgs_final_kernel<<<nb, LB_THREADS, 0, s>>>(st, x, ema, ema_decay, nb);
   STB_CUDA_CHECK(cudaGetLastError());
+  return STB_OK;
+}
+
+int launch_lbfgs_step_banded(void* state, const CommDev& c, float* x, float* ema, float ema_decay, int add_seams,
+                             cudaStream_t s) {
+  const long n = 3l * c.own_rows * c.W;
+  STB_CHECK(n < (1l << 31), STB_ERR_INVALID, "band of %d x %d pixels is too large", c.own_rows, c.W);
+  const LbState st = carve(state, n);
+  const int nb = lb_blocks(n);
+  STB_TRY(launch_lbfgs_seam_gather(c, st.g, add_seams, s));
+  lbfgs_pass0_kernel<<<nb, LB_THREADS, 0, s>>>(st);
+  lbfgs_xreduce_kernel<<<1, LB_THREADS, 0, s>>>(c, st.part0, 4, nb, 1, 0);
+  lbfgs_decide_kernel<<<1, LB_THREADS, 0, s>>>(st, 1);
+  for (int r = 0; r < LB_ROUNDS; ++r) {
+    lbfgs_round_kernel<<<nb, LB_THREADS, 0, s>>>(st, r, 1);
+    lbfgs_xreduce_kernel<<<1, LB_THREADS, 0, s>>>(c, st.part + (r & 1) * LB_MAX_BLOCKS, 1, nb, 0, r + 1);
+  }
+  if (c.W % 4 == 0) lbfgs_final_banded_kernel<4><<<nb, LB_THREADS, 0, s>>>(st, c, x, ema, ema_decay);
+  else lbfgs_final_banded_kernel<1><<<nb, LB_THREADS, 0, s>>>(st, c, x, ema, ema_decay);
+  STB_CUDA_CHECK(cudaGetLastError());
+  return STB_OK;
+}
+
+int preload_lbfgs_kernels() {
+  cudaFuncAttributes fa;
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_pass0_kernel));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_decide_kernel));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_round_kernel));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_xreduce_kernel));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_final_banded_kernel<4>));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, lbfgs_final_banded_kernel<1>));
   return STB_OK;
 }
 

@@ -635,8 +635,12 @@ class StyleTransfer:
                     else:
                         sw, sh = size_to_fit(simg.size, style_size)
                     styles.append((sw, sh, _pil_to_tensor(simg.resize((sw, sh), Image.BICUBIC), dev)))
-                # multi-GPU: tile this scale into horizontal bands (None: too small, every rank runs the whole image)
-                band = D.make_band(ch, self._rank, self._world) if (self._dist and optimizer == 'adam') else None
+                # multi-GPU: tile this scale into horizontal bands (None: too small, every rank runs the whole image).
+                # L-BFGS is tiled only with the exchanges inside the library ('peer'): its step needs 22 cross-rank
+                # reductions per iteration, which run as kernels in the iteration's graph.  Under host-driven NCCL
+                # exchanges every rank runs the whole image.
+                tiled = self._dist and (optimizer == 'adam' or self._comm_mode == 'peer')
+                band = D.make_band(ch, self._rank, self._world) if tiled else None
                 h_loc = band.h_local if band is not None else ch
                 self.model.set_band(False)
                 self._band = None
@@ -658,6 +662,8 @@ class StyleTransfer:
                         lb = D.make_band(lh, self._rank, self._world)
                         end_sizes.append((lb.h_local if lb is not None else lh, lw))
                     self._ensure_peer_memory([(h_loc, cw)] + style_sizes + end_sizes, max(cap_h, h_loc), max(ew, cw))
+                    if optimizer == 'lbfgs' and self._comm_mode != 'peer':   # the peer mapping failed on some rank
+                        band, h_loc = None, ch
                 self.model.ensure_workspace([(h_loc, cw)] + style_sizes)
 
                 self.image = self.model.resize(self.image, (ch, cw), 'bicubic', 'clamp')          # ST:420
@@ -705,7 +711,7 @@ class StyleTransfer:
                             grad = torch.empty_like(self.image)
                 else:
                     lbfgs_state = None   # hand the previous scale's block back before the new one is allocated
-                    lbfgs_state = self._lbfgs_state(ch, cw)
+                    lbfgs_state = self._lbfgs_state(band.own_rows if band is not None else ch, cw)
                 torch.cuda.empty_cache()
 
                 actual_its = initial_iterations if scale == scales[0] else iterations
@@ -716,6 +722,9 @@ class StyleTransfer:
                     elif optimizer == 'adam':
                         step += 1
                         self._iterate(exp_avg, exp_avg_sq, step, step_size, avg_decay, callback is not None)
+                    elif band is not None:
+                        step += 1
+                        self._iterate_lbfgs_banded(lbfgs_state, step, avg_decay)
                     else:
                         step += 1
                         self._iterate_lbfgs(lbfgs_state, step, avg_decay)
@@ -740,7 +749,8 @@ class StyleTransfer:
                     g = self._group
                     self.average = EMA.from_state(D.gather_rows(self.average.value, band, g), self.average.accum,
                                                   avg_decay)
-                    exp_avg, exp_avg_sq = D.gather_rows(exp_avg, band, g), D.gather_rows(exp_avg_sq, band, g)
+                    if optimizer == 'adam':   # L-BFGS starts afresh every scale: it has no state to carry
+                        exp_avg, exp_avg_sq = D.gather_rows(exp_avg, band, g), D.gather_rows(exp_avg_sq, band, g)
                     self.image = self.average.get()
                     self.model.set_band(False)
                 else:
@@ -753,7 +763,8 @@ class StyleTransfer:
     # LBFGS.step (max_iter=1, history_size=10) and the EMA run natively as one CUDA graph per iteration (csrc/lbfgs.cu)
     def _lbfgs_state(self, h, w):
         """Fresh optimizer state for one scale (the reference builds a new optim.LBFGS per scale): a torch-owned block
-        of ~25 x 3HW floats (history ring, g, g_prev, d), so that max_memory_allocated stays truthful."""
+        of ~25 x 3HW floats (history ring, g, g_prev, d), so that max_memory_allocated stays truthful.  On a tiled
+        scale h is the band's own rows: each rank keeps the vectors of its own rows only."""
         lib = self.model.lib
         n = ctypes.c_size_t()
         _lib.check(lib.stb_lbfgs_state_bytes(h, w, ctypes.byref(n)))
@@ -766,4 +777,13 @@ class StyleTransfer:
         m = self.model
         _lib.check(m.lib.stb_iterate_lbfgs(m.ctx, _lib.ptr(self.image), _lib.ptr(self.average.value), _lib.ptr(state),
                                            state.numel(), step, avg_decay, None, _lib.cur_stream()))
+        self.average.note_update()
+
+    def _iterate_lbfgs_banded(self, state, step, avg_decay):
+        """One L-BFGS iteration of a tiled scale ('peer' mode): one CUDA graph with the compute, the exchanges and the
+        cross-rank reductions of the step; the loss goes to the loss ring like the untiled one's."""
+        m = self.model
+        _lib.check(m.lib.stb_iterate_lbfgs_banded(m.ctx, _lib.ptr(self.image), _lib.ptr(self.average.value),
+                                                  _lib.ptr(state), state.numel(), step, avg_decay, None,
+                                                  _lib.cur_stream()))
         self.average.note_update()
