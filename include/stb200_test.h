@@ -54,6 +54,10 @@ STB_API int stb_test_preload(void);
 STB_API int stb_test_lbfgs_step_banded(stb_ctx* ctx, void* state, size_t bytes, float* x, const float* grad,
                                        float* ema, float ema_decay, int add_seams, int* pairs_out, float* t_out,
                                        void* stream);
+/* copy the 3*H*W floats of the gradient the last L-BFGS step consumed out of a state of stb_lbfgs_state_bytes(H, W)
+ * bytes (stream-ordered): after stb_iterate_lbfgs the whole-image closure gradient; after stb_iterate_lbfgs_banded
+ * (H = own rows) the band's own-row gradient after the seam reduce. */
+STB_API int stb_test_lbfgs_gradient(const void* state, size_t bytes, int H, int W, float* out, void* stream);
 
 #ifdef __cplusplus
 }

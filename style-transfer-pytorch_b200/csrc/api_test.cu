@@ -117,6 +117,18 @@ int stb_test_lbfgs_step(void* state, size_t bytes, int H, int W, float* x, const
   return STB_OK;
 }
 
+// The gradient the last L-BFGS step consumed: after stb_iterate_lbfgs the whole-image closure gradient, after
+// stb_iterate_lbfgs_banded (H = own rows) the band's own-row gradient after the seam reduce.
+int stb_test_lbfgs_gradient(const void* state, size_t bytes, int H, int W, float* out, void* stream) {
+  STB_CHECK(state && out && H > 0 && W > 0, STB_ERR_INVALID, "bad argument");
+  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0, STB_ERR_INVALID, "state must be 256-byte aligned");
+  const long n = 3l * H * W;
+  STB_CHECK(bytes >= lbfgs_state_bytes(n), STB_ERR_INVALID, "L-BFGS state too small");
+  STB_CUDA_CHECK(cudaMemcpyAsync(out, lbfgs_grad_buffer(const_cast<void*>(state), n), n * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+  return STB_OK;
+}
+
 // Loads every kernel of THIS library (it holds its own copies of the product kernels).  A banded test step must not be
 // the first launch of a kernel: a lazy module load synchronises the context, which deadlocks against a peer's resident
 // wait kernel (see comm_preload).
