@@ -20,10 +20,28 @@ STB_API int stb_test_pixel_gemm(int H, int W, int Cin, int Cout, int C2, int mod
                                 const void* A2, int a2_row0, int a2_rows, const void* B2, void* out,
                                 const float* bias, const void* mask_src, const void* ctarget, float cscale,
                                 int row_lo, int row_hi, void* stream);
+/* TV loss partials and gradient (times tv_weight) on rows [row0, row0+rows) of the fp32 [3][H][W] image, with the loss
+ * means taken over H_norm rows (a band's global height): gtv [3][H][W] (own rows written), tv_partials
+ * ceil(W/256) * rows floats, one per (row, 256-column block), their count in *n_partials. */
+STB_API int stb_test_tv(const float* img, int H, int W, int row0, int rows, int H_norm, float tv_weight, float* gtv,
+                        float* tv_partials, int* n_partials, void* stream);
+/* conv0 forward, out bf16 [H][W][64]; when gtv is not NULL, first stb_test_tv on the whole image */
 STB_API int stb_test_conv0_fwd(const float* img, const float* w0, const float* b0, void* out_bf16, int H, int W,
                                float tv_weight, float* gtv, float* tv_partials, int* n_partials, void* stream);
+/* conv0 backward as the end of the product's backward pass runs it: the wgmma interior kernel, then the SIMT border
+ * kernel.  g0 bf16 [H][W][64], gtv (optional) and grad_out (optional) fp32 [3][H][W].  apply_update: both kernels also
+ * take the Adam + clamp + EMA step of Adam step `step` on img / exp_avg / exp_avg_sq / ema (fp32 [3][H][W]). */
+STB_API int stb_test_conv0_bwd_adam(const void* g0_bf16, const float* w0, const float* gtv, float* grad_out, int H,
+                                    int W, float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step,
+                                    float lr, float beta1, float beta2, float eps, float ema_decay, int apply_update,
+                                    void* stream);
+/* stb_test_conv0_bwd_adam without the update */
 STB_API int stb_test_conv0_bwd(const void* g0_bf16, const float* w0, const float* gtv, float* grad_out, int H, int W,
                                void* stream);
+/* content SSE partials: sum((a - b)^2) over n bf16 elements (n a multiple of 8, else STB_ERR_INVALID), at most 1024
+ * partials, their count in *n_partials. */
+STB_API int stb_test_sse(const void* a_bf16, const void* b_bf16, long n, float* partials, int* n_partials,
+                         void* stream);
 /* conv 3x3 + bias + ReLU with the 2x2 pool fused into its epilogue (the product's only pool-forward path):
  * out [H][W][Cout] and pool_out [H/2][W/2][Cout], both bf16 NHWC. */
 STB_API int stb_test_conv_pool(int H, int W, int Cin, int Cout, const void* A, const void* Bw, const float* bias,

@@ -85,7 +85,10 @@ def _declare_test(lib):
         'stb_pack_weights': [vp, vp, i, i, i, vp],
         'stb_test_pixel_gemm': [i, i, i, i, i, i, vp, vp, vp, i, i, vp, vp, vp, vp, vp, f, i, i, vp],
         'stb_test_conv0_fwd': [vp, vp, vp, vp, i, i, f, vp, vp, C.POINTER(i), vp],
+        'stb_test_tv': [vp, i, i, i, i, i, f, vp, vp, C.POINTER(i), vp],
         'stb_test_conv0_bwd': [vp, vp, vp, vp, i, i, vp],
+        'stb_test_conv0_bwd_adam': [vp, vp, vp, vp, i, i, vp, vp, vp, vp, C.c_int64, f, f, f, f, f, i, vp],
+        'stb_test_sse': [vp, vp, C.c_long, vp, C.POINTER(i), vp],
         'stb_test_conv_pool': [i, i, i, i, vp, vp, vp, vp, vp, i, vp],
         'stb_test_pool_bwd': [i, vp, vp, vp, i, i, i, vp],
         'stb_test_gram': [vp, C.c_long, i, vp, sz, vp, vp, vp],
@@ -115,9 +118,9 @@ EXPORTS = [
 ]
 # include/stb200_test.h (libstb200_test.so)
 TEST_EXPORTS = [
-    'stb_test_last_error', 'stb_pack_weights', 'stb_test_pixel_gemm', 'stb_test_conv0_fwd', 'stb_test_conv0_bwd',
-    'stb_test_conv_pool', 'stb_test_pool_bwd', 'stb_test_gram', 'stb_test_gram_partials_floats', 'stb_test_w2',
-    'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step', 'stb_test_lbfgs_step_banded',
+    'stb_test_last_error', 'stb_pack_weights', 'stb_test_pixel_gemm', 'stb_test_conv0_fwd', 'stb_test_tv',
+    'stb_test_conv0_bwd', 'stb_test_conv0_bwd_adam', 'stb_test_sse', 'stb_test_conv_pool', 'stb_test_pool_bwd', 'stb_test_gram',
+    'stb_test_gram_partials_floats', 'stb_test_w2', 'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step', 'stb_test_lbfgs_step_banded',
     'stb_test_lbfgs_gradient', 'stb_test_preload',
 ]
 

@@ -372,17 +372,6 @@ __global__ void adam_scalars_kernel(long long* step, AdamScalars* out, float lr,
   *out = as;
 }
 
-AdamScalars make_adam_scalars(int64_t step, float lr, float beta1, float beta2, float adam_eps, float ema_decay) {
-  AdamScalars as{};
-  const double bc1 = 1.0 - std::pow((double)beta1, (double)step);
-  const double bc2 = 1.0 - std::pow((double)beta2, (double)step);
-  as.one_minus_b1 = 1.f - beta1; as.b2 = beta2; as.one_minus_b2 = 1.f - beta2;
-  as.step_size = (float)((double)lr / bc1);
-  as.inv_sqrt_bc2 = (float)(1.0 / std::sqrt(bc2));
-  as.eps = adam_eps; as.ema_decay = ema_decay; as.one_minus_decay = 1.f - ema_decay;
-  return as;
-}
-
 // the iteration counter of the loss ring's stamps on a path without Adam scalars (stb_iterate_lbfgs)
 __global__ void advance_step_kernel(long long* step) { *step += 1; }
 
@@ -420,6 +409,17 @@ __global__ void finalize_loss_kernel(const float* __restrict__ scalars, float co
 }
 
 }  // namespace
+
+AdamScalars stb::make_adam_scalars(int64_t step, float lr, float beta1, float beta2, float adam_eps, float ema_decay) {
+  AdamScalars as{};
+  const double bc1 = 1.0 - std::pow((double)beta1, (double)step);
+  const double bc2 = 1.0 - std::pow((double)beta2, (double)step);
+  as.one_minus_b1 = 1.f - beta1; as.b2 = beta2; as.one_minus_b2 = 1.f - beta2;
+  as.step_size = (float)((double)lr / bc1);
+  as.inv_sqrt_bc2 = (float)(1.0 / std::sqrt(bc2));
+  as.eps = adam_eps; as.ema_decay = ema_decay; as.one_minus_decay = 1.f - ema_decay;
+  return as;
+}
 
 namespace {
 void comm_release(stb_ctx* ctx) {

@@ -40,11 +40,21 @@ int stb_test_pixel_gemm(int H, int W, int Cin, int Cout, int C2, int mode, const
 
 extern "C" {
 
+int stb_test_tv(const float* img, int H, int W, int row0, int rows, int H_norm, float tv_weight, float* gtv,
+                float* tv_partials, int* n_partials, void* stream) {
+  STB_CHECK(img && gtv && tv_partials && H > 0 && W > 0 && H_norm > 0, STB_ERR_INVALID, "bad argument");
+  STB_CHECK(row0 >= 0 && rows > 0 && row0 + rows <= H, STB_ERR_INVALID, "row window [%d, %d) outside 0..%d", row0,
+            row0 + rows, H);
+  return launch_tv(img, H, W, row0, rows, H_norm, tv_weight, gtv, tv_partials, n_partials,
+                   static_cast<cudaStream_t>(stream));
+}
+
 int stb_test_conv0_fwd(const float* img, const float* w0, const float* b0, void* out_bf16, int H, int W,
                        float tv_weight, float* gtv, float* tv_partials, int* n_partials, void* stream) {
-  // product path of conv0: TV kernel and the fused im2col + wgmma GEMM + bias + ReLU kernel
+  // product path of conv0: TV on the whole image (when gtv is given) and the fused im2col + wgmma GEMM + bias + ReLU
+  // kernel
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (gtv != nullptr) STB_TRY(launch_tv(img, H, W, 0, H, H, tv_weight, gtv, tv_partials, n_partials, s));
+  if (gtv != nullptr) STB_TRY(stb_test_tv(img, H, W, 0, H, H, tv_weight, gtv, tv_partials, n_partials, stream));
   bf16* wp = nullptr;
   STB_CUDA_CHECK(cudaMalloc(&wp, 64 * 64 * 2));
   int rc = pack_weights_conv0_fwd(w0, wp, s);
@@ -54,22 +64,46 @@ int stb_test_conv0_fwd(const float* img, const float* w0, const float* b0, void*
   return rc;
 }
 
-int stb_test_conv0_bwd(const void* g0_bf16, const float* w0, const float* gtv, float* grad_out, int H, int W,
-                       void* stream) {
-  // product path: interior via the wgmma 1x1 GEMM + col2im kernel with the image-space epilogue, borders in SIMT
+int stb_test_conv0_bwd_adam(const void* g0_bf16, const float* w0, const float* gtv, float* grad_out, int H, int W,
+                            float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step, float lr,
+                            float beta1, float beta2, float eps, float ema_decay, int apply_update, void* stream) {
+  // the tail of the product's backward pass: interior via the wgmma 1x1 GEMM + col2im kernel with the image-space
+  // epilogue, then the border ring in SIMT, each with the fused Adam + clamp + EMA step when apply_update
+  STB_CHECK(!apply_update || (img && exp_avg && exp_avg_sq && ema && step >= 1), STB_ERR_INVALID,
+            "apply_update needs img, exp_avg, exp_avg_sq, ema and step >= 1");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   bf16* wp = nullptr;
+  AdamScalars* d_adam = nullptr;
   STB_CUDA_CHECK(cudaMalloc(&wp, 32 * 64 * 2));
-  int rc = pack_weights_conv0_bwd(w0, wp, s);
+  int rc = STB_OK;
+  if (apply_update) {
+    const AdamScalars as = make_adam_scalars(step, lr, beta1, beta2, eps, ema_decay);
+    if (cudaMalloc(&d_adam, sizeof(AdamScalars)) != cudaSuccess ||
+        cudaMemcpyAsync(d_adam, &as, sizeof(AdamScalars), cudaMemcpyHostToDevice, s) != cudaSuccess)
+      rc = set_error(STB_ERR_CUDA, "conv0 bwd: Adam scalars to the device");
+  }
+  if (rc == 0) rc = pack_weights_conv0_bwd(w0, wp, s);
   if (rc == 0)
-    rc = launch_conv0_bwd_interior(static_cast<const bf16*>(g0_bf16), wp, gtv, nullptr, nullptr, nullptr, nullptr,
-                                   grad_out, H, W, nullptr, 0, s);
+    rc = launch_conv0_bwd_interior(static_cast<const bf16*>(g0_bf16), wp, gtv, img, exp_avg, exp_avg_sq, ema,
+                                   grad_out, H, W, d_adam, apply_update, s);
   if (rc == 0)
-    rc = launch_conv0_bwd_adam(static_cast<const bf16*>(g0_bf16), true, w0, gtv, nullptr, nullptr, nullptr, nullptr,
-                               grad_out, H, W, nullptr, 0, s);
+    rc = launch_conv0_bwd_adam(static_cast<const bf16*>(g0_bf16), true, w0, gtv, img, exp_avg, exp_avg_sq, ema,
+                               grad_out, H, W, d_adam, apply_update, s);
   cudaStreamSynchronize(s);
   cudaFree(wp);
+  if (d_adam) cudaFree(d_adam);
   return rc;
+}
+
+int stb_test_conv0_bwd(const void* g0_bf16, const float* w0, const float* gtv, float* grad_out, int H, int W,
+                       void* stream) {
+  return stb_test_conv0_bwd_adam(g0_bf16, w0, gtv, grad_out, H, W, nullptr, nullptr, nullptr, nullptr, 0, 0.f, 0.f,
+                                 0.f, 0.f, 0.f, 0, stream);
+}
+
+int stb_test_sse(const void* a_bf16, const void* b_bf16, long n, float* partials, int* n_partials, void* stream) {
+  return launch_sse(static_cast<const bf16*>(a_bf16), static_cast<const bf16*>(b_bf16), n, partials, n_partials,
+                    static_cast<cudaStream_t>(stream));
 }
 
 int stb_test_conv_pool(int H, int W, int Cin, int Cout, const void* A, const void* Bw, const float* bias, void* out,

@@ -498,6 +498,8 @@ int preload_image_kernels() {
 }
 
 int launch_sse(const bf16* a, const bf16* b, long n, float* partials, int* n_partials, cudaStream_t s) {
+  // the kernel reads 8 elements per 16-byte load: a remainder would be silently left out of the sum
+  STB_CHECK(n >= 0 && n % 8 == 0, STB_ERR_INVALID, "sse: n = %ld is not a multiple of 8", n);
   const long n8 = n / 8;
   int g = grid_for(n8, 256);
   if (g > 1024) g = 1024;

@@ -48,6 +48,8 @@ int pack_weights_bwd(const float* w, bf16* out, int Cout, int Cin, cudaStream_t 
 struct AdamScalars {  // torch/optim/adam.py:413-546 scalars, evaluated on the host in double like torch does
   float one_minus_b1, b2, one_minus_b2, step_size, inv_sqrt_bc2, eps, ema_decay, one_minus_decay;
 };
+// the scalars of Adam step `step` (1-based), as the host-side update paths evaluate them (api.cu)
+AdamScalars make_adam_scalars(int64_t step, float lr, float beta1, float beta2, float adam_eps, float ema_decay);
 // TV loss partials + gradient (times tv_weight) on the raw image; weights of the tensor-core conv0 in its split
 // K layout (27 hi taps, 27 lo residuals, 10 zeros).
 int launch_tv(const float* img, int H, int W, int row0, int rows, int H_norm, float tv_weight, float* gtv,
