@@ -14,7 +14,9 @@
 //               per 64-channel chunk it loads three "dx buffers" (18 rows x 8 px x 64 ch, SW128,
 //               zero-filled out of bounds = the conv's zero padding); the three dy taps are 1 KiB-aligned row
 //               shifts inside a dx buffer, so each activation byte is fetched 3.4x instead of 9x from L2.
-//               Weights stream tap by tap through a second ring.
+//               Weights stream tap by tap through a second ring.  In dgrad (MODE 1) the epilogue operands, the
+//               ReLU mask and the content target, follow a tile's K stages through the A ring, one box per
+//               64-channel output chunk (or the staged tap operand A2 is kept as the mask when it is the mask).
 //   warps 0-7   two consumer warpgroups: warpgroup g owns pixel rows 8g .. 8g+7 of every sub-tile (M = 64), issues
 //               its wgmma (bf16 x bf16 -> fp32 registers, one MMA group in flight while the next is issued), then
 //               runs the epilogue: bias/ReLU or mask/content -> bf16 -> swizzled smem -> TMA store (+ fused pool).
@@ -68,6 +70,7 @@ struct KParams {
   int row_lo, row_hi;
   int pooling;  // MODE 0: -1 = none, else STB_POOL_*: also emit the 2x2-pooled output (tmPool)
   int y_origin; // first output row of the tile grid (row window of a band that computes its own rows only)
+  int mask_reuse; // MODE 1: the A2 chunks of a tile are its mask chunks; keep them in the ring for the epilogue
 };
 
 template <int BN, int MODE>
@@ -75,6 +78,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                   const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmPool,
+                  const __grid_constant__ CUtensorMap tmMask, const __grid_constant__ CUtensorMap tmCt,
                   const KParams p) {
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
@@ -100,6 +104,8 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmB2);
     tma_prefetch_desc(&tmOut);
     tma_prefetch_desc(&tmPool);
+    tma_prefetch_desc(&tmMask);
+    tma_prefetch_desc(&tmCt);
     // empty barriers: one arrival per consumer warp once its wgmma reads of the stage are complete
     for (int i = 0; i < C::NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
     for (int i = 0; i < C::NB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 8); }
@@ -149,6 +155,24 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           tma_load_3d(smem + C::OFF_B + sb * C::B_STAGE_BYTES, &tmB2, &b_full[sb], c * 64, n0, 0);
           if (++sb == C::NB) { sb = 0; pb ^= 1; }
         }
+        // MODE 1 epilogue operands: per 64-channel output chunk j, the mask box (unless the A2 chunks just loaded
+        // are the mask) and on the content layer the content-target box, both at the output tile's coordinates and
+        // zero-filled outside the image.  The consumers walk the same sequence: K stages, C2 stages, then these.
+        // No deadlock: the slot a chunk needs last held either a K / C2 stage, which the consumers release at the
+        // latest with the final MMA wait before the epilogue, or an earlier epilogue chunk, which they release once
+        // that chunk is stored; neither release waits on a load issued after it.  Held A2 chunks (mask_reuse) are
+        // at most NA - 1 with a content target, so a target chunk always finds a slot that frees.
+        if (MODE == 1) {
+          for (int j = 0; j < BN / 64; ++j) {
+            for (int t = p.mask_reuse ? 1 : 0; t < (p.ctarget != nullptr ? 2 : 1); ++t) {
+              mbar_wait(&a_empty[sa], pa ^ 1);
+              mbar_expect_tx(&a_full[sa], C::A2_BYTES);
+              tma_load_3d(smem + C::OFF_A + sa * C::A_STAGE_BYTES, t ? &tmCt : &tmMask, &a_full[sa], n0 + j * 64, x0,
+                          y0);
+              if (++sa == C::NA) { sa = 0; pa ^= 1; }
+            }
+          }
+        }
       }
     }
     __syncwarp();
@@ -161,6 +185,7 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const uint32_t bar0 = 1 + 3 * wg;              // named barriers of this warpgroup
     const uint32_t a_base0 = smem_u32(smem + C::OFF_A) + wg * HALF_H * C::A_PITCH;
     const uint32_t b_base0 = smem_u32(smem + C::OFF_B);
+    const uint32_t a_ring = smem_u32(smem + C::OFF_A);  // MODE 1 epilogue operands are read from here
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
     int stg = 0;
@@ -208,10 +233,12 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (++sa == C::NA) { sa = 0; pa ^= 1; }
         }
       }
+      const bool reuse = MODE == 1 && p.mask_reuse;
+      const int sa2 = sa;  // ring slot of A2 chunk 0; with mask_reuse, A2 chunk j stays there as mask chunk j
       for (int c = 0; c < n_chunks2; ++c) {
         mbar_wait(&a_full[sa], pa);
         mbar_wait(&b_full[sb], pb);
-        mma_stage(a_base0 + sa * C::A_STAGE_BYTES, sb, sa);
+        mma_stage(a_base0 + sa * C::A_STAGE_BYTES, sb, reuse ? -1 : sa);
         if (++sb == C::NB) { sb = 0; pb ^= 1; }
         if (++sa == C::NA) { sa = 0; pa ^= 1; }
       }
@@ -219,14 +246,33 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
       for (int m = 0; m < C::MT; ++m) wgmma_fence_acc(acc[m]);
 
-      // ---- epilogue: this warpgroup's 8 x 8 pixels of sub-tile m, 64 channels (j) at a time
+      // ---- epilogue: this warpgroup's 8 x 8 pixels of sub-tile m, 64 channels (j) at a time.  MODE 1 walks the
+      // chunks j outermost, so that each mask / content-target chunk in the A ring is read by every sub-tile and
+      // then released; the other modes walk the sub-tiles outermost.
       const int rr = wq * 16 + (lane >> 2);        // pixel (row) of the first accumulator row held by this thread
       const int cq = 2 * (lane & 3);               // first of the two columns held per 8-column group
+      constexpr int NJ = BN / 64;
+      int mslot = 0, tslot = 0;                    // MODE 1: A ring slots of chunk j's mask and content target
 #pragma unroll
-      for (int m = 0; m < C::MT; ++m) {
+      for (int e = 0; e < C::MT * NJ; ++e) {
+        const int m = MODE == 1 ? e % C::MT : e / NJ;
+        const int j = MODE == 1 ? e / C::MT : e % NJ;
         const int x0 = (tx * C::MT + m) * TILE_W;
-#pragma unroll
-        for (int j = 0; j < BN / 64; ++j) {
+        if (MODE == 1 && m == 0) {
+          if (reuse) {
+            mslot = (sa2 + j) % C::NA;
+          } else {
+            mslot = sa;
+            mbar_wait(&a_full[sa], pa);
+            if (++sa == C::NA) { sa = 0; pa ^= 1; }
+          }
+          if (p.ctarget != nullptr) {
+            tslot = sa;
+            mbar_wait(&a_full[sa], pa);
+            if (++sa == C::NA) { sa = 0; pa ^= 1; }
+          }
+        }
+        {
           uint8_t* stage = smem + C::OFF_STG + (2 * wg + stg) * STG_BYTES;
           // make sure the TMA store that last read this staging buffer is done, then let everyone write
           if (et == 0) tma_store_wait_read<1>();
@@ -238,7 +284,10 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const bool inb = (py < p.H) && (px < p.W);
             const bool in_rows = (py >= p.row_lo) && (py < p.row_hi);
             const bool has_c = (p.ctarget != nullptr) && in_rows && inb;
-            const size_t pix_off = (static_cast<size_t>(py) * p.W + px) * p.Cout + n0 + j * 64 + cq;
+            // pixel r of sub-tile m in a [TILE_H][8 MT][64 ch] SW128 box of the A ring (MODE 1 operands)
+            const int box_off = ((wg * HALF_H + (r >> 3)) * TILE_W * C::MT + m * TILE_W + (r & 7)) * 128 + cq * 2;
+            const uint32_t mrow = a_ring + mslot * C::A_STAGE_BYTES + box_off;
+            const uint32_t trow = a_ring + tslot * C::A_STAGE_BYTES + box_off;
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
               const int cb = j * 64 + q * 8 + cq;    // column inside the N tile
@@ -249,14 +298,14 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               } else if (MODE == 2) {
                 packed = pack_bf16x2(a, b);
               } else {
-                const uint32_t yw = inb ? __ldg(reinterpret_cast<const unsigned*>(p.mask_src + pix_off + q * 8)) : 0u;
+                const uint32_t yw = lds_u32(mrow + ((q ^ (r & 7)) << 4));
                 const float ya = bf16lo(yw), yb = bf16hi(yw);
                 if (in_rows) {
                   a += s_bias[n0 + cb];
                   b += s_bias[n0 + cb + 1];
                 }
                 if (has_c) {
-                  const uint32_t tw = __ldg(reinterpret_cast<const unsigned*>(p.ctarget + pix_off + q * 8));
+                  const uint32_t tw = lds_u32(trow + ((q ^ (r & 7)) << 4));
                   a += p.cscale * (ya - bf16lo(tw));
                   b += p.cscale * (yb - bf16hi(tw));
                 }
@@ -268,6 +317,11 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
           fence_proxy_async_smem();
           named_bar_sync(bar0 + 1, 128);
+          if (MODE == 1 && m == C::MT - 1 && lane == 0) {
+            // the warp's reads of chunk j's operands are done (they fed the staging writes): hand the slots back
+            mbar_arrive(&a_empty[mslot]);
+            if (p.ctarget != nullptr) mbar_arrive(&a_empty[tslot]);
+          }
           const bool pooled = (MODE == 0) && p.pooling >= 0;
           if (et == 0) {
             tma_store_3d(&tmOut, stage, n0 + j * 64, x0, y0);
@@ -326,7 +380,8 @@ pixel_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 template <int BN, int MODE>
 int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
-               const CUtensorMap& tmOut, const CUtensorMap& tmPool, const KParams& kp, cudaStream_t stream) {
+               const CUtensorMap& tmOut, const CUtensorMap& tmPool, const CUtensorMap& tmMask, const CUtensorMap& tmCt,
+               const KParams& kp, cudaStream_t stream) {
   using C = Cfg<BN>;
   auto kern = pixel_gemm_kernel<BN, MODE>;
   STB_TRY(ensure_dynamic_smem(reinterpret_cast<const void*>(kern), C::SMEM_BYTES));
@@ -344,7 +399,7 @@ int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = pdl ? 1 : 0;
-  STB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp));
+  STB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp));
   return STB_OK;
 }
 
@@ -376,11 +431,29 @@ int launch_pixel_gemm(const PixelGemmArgs& a, cudaStream_t stream) {
   STB_CHECK(a.mode >= 0 && a.mode <= 2, STB_ERR_INVALID, "pixel_gemm: mode=%d", a.mode);
   if (a.mode == 1) STB_CHECK(a.mask_src != nullptr, STB_ERR_INVALID, "pixel_gemm: bwd needs mask_src");
 
-  CUtensorMap tmA, tmB, tmA2, tmB2, tmOut, tmPool;
+  // The tap operand is the mask itself on the 64- and 128-channel style taps (A2 = the tap's activation, which the
+  // dgrad masks): its chunks, staged in the A ring for the C2 GEMM, then serve as the mask chunks.  Only where A2
+  // holds the mask at every row the tiles store: a band computing its aprons (y_origin below the A2 window) sees A2
+  // zero-filled there, so it streams the mask; and the held chunks must leave a ring slot for the content target.
+  const int a2_rows = a.a2_rows > 0 ? a.a2_rows : a.H;
+  const int y_end = a.y_origin + kp.tiles_y * TILE_H < a.H ? a.y_origin + kp.tiles_y * TILE_H : a.H;
+  kp.mask_reuse = a.mode == 1 && a.C2 == a.Cout && BN == a.Cout && a.A2 != nullptr &&
+                  a.A2 == a.mask_src + static_cast<size_t>(a.a2_row0) * a.W * a.C2 &&
+                  a.C2 / 64 + (a.ctarget != nullptr) <= Cfg<64>::NA && a.a2_row0 <= a.y_origin &&
+                  a.a2_row0 + a2_rows >= y_end;
+  static_assert(Cfg<64>::NA == Cfg<128>::NA, "one A ring depth for the reusable widths");
+
+  CUtensorMap tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt;
   const uint64_t W = a.W, H = a.H;
   // output first; unused maps alias it so that every descriptor handed to the kernel is valid
   STB_TRY(make_tmap_bf16_3d(&tmOut, a.out, a.Cout, W, H, a.Cout * 2ull, W * a.Cout * 2ull, 64, TILE_W, HALF_H));
-  tmA = tmB = tmA2 = tmB2 = tmPool = tmOut;
+  tmA = tmB = tmA2 = tmB2 = tmPool = tmMask = tmCt = tmOut;
+  if (a.mode == 1) {
+    // epilogue operands, [H][W][Cout], loaded per output tile and 64-channel chunk in the A2 box geometry
+    STB_TRY(make_tmap_bf16_3d(&tmMask, a.mask_src, a.Cout, W, H, a.Cout * 2ull, W * a.Cout * 2ull, 64, tile_w, TILE_H));
+    if (a.ctarget != nullptr)
+      STB_TRY(make_tmap_bf16_3d(&tmCt, a.ctarget, a.Cout, W, H, a.Cout * 2ull, W * a.Cout * 2ull, 64, tile_w, TILE_H));
+  }
   kp.pooling = -1;
   if (a.pool_out != nullptr) {
     STB_CHECK(a.mode == 0 && a.pooling >= 0 && a.pooling <= 2 && H >= 2 && W >= 2, STB_ERR_INVALID,
@@ -399,17 +472,17 @@ int launch_pixel_gemm(const PixelGemmArgs& a, cudaStream_t stream) {
     STB_TRY(make_tmap_bf16_3d(&tmB2, a.B2, a.C2, a.Cout, 1, a.C2 * 2ull, (uint64_t)a.Cout * a.C2 * 2ull, 64, BN, 1));
   }
   if (a.mode == 0) {
-    if (BN == 256) return launch_cfg<256, 0>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
-    if (BN == 128) return launch_cfg<128, 0>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
-    return launch_cfg<64, 0>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
+    if (BN == 256) return launch_cfg<256, 0>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
+    if (BN == 128) return launch_cfg<128, 0>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
+    return launch_cfg<64, 0>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
   } else if (a.mode == 1) {
-    if (BN == 256) return launch_cfg<256, 1>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
-    if (BN == 128) return launch_cfg<128, 1>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
-    return launch_cfg<64, 1>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
+    if (BN == 256) return launch_cfg<256, 1>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
+    if (BN == 128) return launch_cfg<128, 1>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
+    return launch_cfg<64, 1>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
   } else {
-    if (BN == 256) return launch_cfg<256, 2>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
-    if (BN == 128) return launch_cfg<128, 2>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
-    return launch_cfg<64, 2>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, kp, stream);
+    if (BN == 256) return launch_cfg<256, 2>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
+    if (BN == 128) return launch_cfg<128, 2>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
+    return launch_cfg<64, 2>(tmA, tmB, tmA2, tmB2, tmOut, tmPool, tmMask, tmCt, kp, stream);
   }
 }
 
