@@ -76,6 +76,10 @@ STB_API int stb_test_lbfgs_step_banded(stb_ctx* ctx, void* state, size_t bytes, 
  * bytes (stream-ordered): after stb_iterate_lbfgs the whole-image closure gradient; after stb_iterate_lbfgs_banded
  * (H = own rows) the band's own-row gradient after the seam reduce. */
 STB_API int stb_test_lbfgs_gradient(const void* state, size_t bytes, int H, int W, float* out, void* stream);
+/* on a context with comm connection and geometry set: *pdl_out = 1 when its exchange kernels launch their successors
+ * early (one process per GPU, stb_comm_connect_ipc, or in-process ranks on pairwise distinct devices); the devices of
+ * its own mailbox and of its own peer-mapped workspace (-1 when it has none: apron mode) */
+STB_API int stb_test_comm_info(stb_ctx* ctx, int* pdl_out, int* mailbox_device_out, int* workspace_device_out);
 
 #ifdef __cplusplus
 }

@@ -96,6 +96,7 @@ def _declare_test(lib):
         'stb_test_lbfgs_step': [vp, sz, i, i, vp, vp, vp, f, C.POINTER(i), C.POINTER(f), vp],
         'stb_test_lbfgs_step_banded': [vp, vp, sz, vp, vp, vp, f, i, C.POINTER(i), C.POINTER(f), vp],
         'stb_test_lbfgs_gradient': [vp, sz, i, i, vp, vp],
+        'stb_test_comm_info': [vp, C.POINTER(i), C.POINTER(i), C.POINTER(i)],
     })
     lib.stb_test_preload.argtypes = []
     lib.stb_test_preload.restype = C.c_int
@@ -121,7 +122,7 @@ TEST_EXPORTS = [
     'stb_test_last_error', 'stb_pack_weights', 'stb_test_pixel_gemm', 'stb_test_conv0_fwd', 'stb_test_tv',
     'stb_test_conv0_bwd', 'stb_test_conv0_bwd_adam', 'stb_test_sse', 'stb_test_conv_pool', 'stb_test_pool_bwd', 'stb_test_gram',
     'stb_test_gram_partials_floats', 'stb_test_w2', 'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step', 'stb_test_lbfgs_step_banded',
-    'stb_test_lbfgs_gradient', 'stb_test_preload',
+    'stb_test_lbfgs_gradient', 'stb_test_preload', 'stb_test_comm_info',
 ]
 
 

@@ -86,7 +86,11 @@ def main(argv=None):
         devices = [torch.device('cuda:0')]
     if len(set(d.type for d in devices)) != 1 or devices[0].type != 'cuda':
         sys.exit('devices must all be CUDA devices')
-    print('GPU 0 type:' if len(devices) == 1 else 'GPU types:', *(torch.cuda.get_device_name(d) for d in devices))
+    # two devices in one process: StyleTransfer runs one rank per device and tiles the large scales across them
+    for i, device in enumerate(devices):
+        props = torch.cuda.get_device_properties(device)
+        print(f'GPU {i} type: {props.name} (compute {props.major}.{props.minor})')
+        print(f'GPU {i} RAM:', round(props.total_memory / 1024 / 1024), 'MB')
 
     end_scale = str(args.end_scale)
     if end_scale.endswith('+'):  # "N+": a safe scale for a non-square image given that N x N fits (CLI:84-87)

@@ -1085,28 +1085,34 @@ int stb_comm_connect_ipc(stb_ctx* ctx, const void* handles) {
   return STB_OK;
 }
 
-// same process (several contexts / streams, e.g. the single-GPU emulation of the tests): plain device pointers
+// same process (several contexts / streams: StyleTransfer(devices=[a, b]), or the single-GPU emulation of the tests):
+// plain device pointers
 int stb_comm_connect_local(stb_ctx* ctx, void* const* mailboxes) {
   STB_ENTER(ctx);
   STB_CHECK(ctx->comm_mailbox && mailboxes, STB_ERR_STATE, "stb_comm_create first");
+  int dev[COMM_MAX_RANKS];
   for (int r = 0; r < ctx->comm.world; ++r) {
     STB_CHECK(mailboxes[r] != nullptr, STB_ERR_INVALID, "null mailbox of rank %d", r);
+    dev[r] = ctx->device;
     if (r == ctx->comm.rank) STB_CHECK(mailboxes[r] == ctx->comm_mailbox, STB_ERR_INVALID, "own mailbox mismatch");
     else {
-      int peer_dev = -1;
       cudaPointerAttributes pa;
       STB_CUDA_CHECK(cudaPointerGetAttributes(&pa, mailboxes[r]));
-      peer_dev = pa.device;
-      if (peer_dev != ctx->device) {
-        cudaError_t e = cudaDeviceEnablePeerAccess(peer_dev, 0);
+      dev[r] = pa.device;
+      if (dev[r] != ctx->device) {
+        cudaError_t e = cudaDeviceEnablePeerAccess(dev[r], 0);
         if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
         else STB_CUDA_CHECK(e);
       }
     }
     ctx->comm.mbox[r] = static_cast<uint8_t*>(mailboxes[r]);
   }
+  // early release is safe only when every rank owns its GPU (see CommDev::pdl): ranks sharing a device keep it off
+  int distinct = 1;
+  for (int a = 0; a < ctx->comm.world; ++a)
+    for (int b = a + 1; b < ctx->comm.world; ++b) distinct = distinct && dev[a] != dev[b];
   ctx->comm_ready = true;
-  ctx->comm.pdl = 0;   // ranks may share a device (see CommDev::pdl)
+  ctx->comm.pdl = distinct;
   return STB_OK;
 }
 

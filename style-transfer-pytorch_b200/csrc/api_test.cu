@@ -195,6 +195,25 @@ int stb_test_lbfgs_step_banded(stb_ctx* ctx, void* state, size_t bytes, float* x
   return STB_OK;
 }
 
+// whether the exchange kernels of a connected context release their dependents early (CommDev::pdl), and the devices
+// that hold its own mailbox and its own peer-mapped workspace (-1: none)
+int stb_test_comm_info(stb_ctx* ctx, int* pdl_out, int* mailbox_device_out, int* workspace_device_out) {
+  STB_CHECK(ctx && pdl_out && mailbox_device_out && workspace_device_out, STB_ERR_INVALID, "null argument");
+  const CommDev* c = ctx_comm(ctx);
+  STB_CHECK(c != nullptr, STB_ERR_STATE, "stb_comm_connect_* + stb_comm_set_geometry first");
+  *pdl_out = c->pdl;
+  const void* own[2] = {c->mbox[c->rank], c->ws[c->rank]};
+  int* out[2] = {mailbox_device_out, workspace_device_out};
+  for (int i = 0; i < 2; ++i) {
+    *out[i] = -1;
+    if (own[i] == nullptr) continue;
+    cudaPointerAttributes pa;
+    STB_CUDA_CHECK(cudaPointerGetAttributes(&pa, own[i]));
+    *out[i] = pa.device;
+  }
+  return STB_OK;
+}
+
 size_t stb_test_w2_workspace_bytes(void) { return W2Engine::workspace_bytes(); }
 
 // Runs the W2 engine with the given problem placed in the slot of matching size (other slots get a benign

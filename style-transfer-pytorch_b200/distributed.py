@@ -13,12 +13,14 @@ Default ("peer" mode): all three run INSIDE the library, as kernels that read th
 IPC peer memory, csrc/comm.cu), so an iteration is one CUDA graph per rank -- `stb_iterate_banded`.  Fallback ("nccl"
 mode, `STB_COMM=nccl` or when the peer mapping cannot be set up): the host drives `stb_iterate_fwd` -> NCCL all-reduce
 -> `stb_iterate_bwd` -> NCCL send/recv -> `stb_adam_update` (exchange_add_grad / exchange_halo below).
-The reference's own multi-device mode (a 2-GPU layer split, ST:326-333) is superseded by this.
+The reference's own multi-device call, `StyleTransfer(devices=[a, b])` (a 2-GPU layer split, ST:326-333), runs this
+tiling instead: one rank per listed device, as threads of the calling process (StyleTransfer._stylize_devices), with
+the exchanges inside the library.
 
 Collectives that are per SCALE, not per iteration (mailbox handle exchange, barriers, tiled style statistics, the
 final gather of the bands) go through a small group interface: `TorchGroup` (torch.distributed, one process per GPU)
-or `ThreadGroup` (the ranks are threads of one process sharing one GPU -- how the test-suite runs the very same tiled
-path on a single-GPU box).
+or `ThreadGroup` (the ranks are threads of one process, each with its own device or all on one -- the two-device
+`StyleTransfer`, and how the test-suite runs the very same tiled path on a single-GPU box).
 """
 from __future__ import annotations
 
@@ -120,7 +122,7 @@ class TorchGroup:
 
 
 class ThreadGroup:
-    """The ranks are THREADS of one process (each with its own context and stream, usually on the same GPU): the
+    """The ranks are THREADS of one process (each with its own context and stream, on its own GPU or sharing one): the
     per-scale collectives go through shared host state; tensors handed over are synchronised on the producer's
     stream first.  Build one `ThreadGroup.Shared(world)` and give `ThreadGroup(shared, rank)` to every thread."""
     peer_kind = 'local'

@@ -9,8 +9,12 @@ the iteration loop (ST:472-486) runs in the native library.  There is no CPU or 
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
+import gc
 import os
+import signal
+import threading
 import time
 import warnings
 from dataclasses import dataclass
@@ -297,6 +301,126 @@ class NativeVGG:
                                             tv_weight, eps, _lib.cur_stream()))
 
 
+class _Stopped(Exception):
+    """The other in-process rank stopped (its error is the one stylize() raises)."""
+
+
+class _PeerUnavailable(Exception):
+    """The in-process ranks could not map each other's memory: the job runs untiled on the first device instead."""
+
+
+class _Lockstep:
+    """Host-side handshake of the two in-process ranks of StyleTransfer(devices=[a, b]), one per stylize() call.
+
+    A banded iteration waits on the device for its peer's stamps, so an iteration launched by one rank and never by the
+    other traps after the exchange timeout.  Both ranks must therefore launch the same steps however either one stops:
+      * rank 1 announces step s (ready1) only once nothing but its launch is left before it: rank 0's callback of step
+        s-1 is over, and with it every gather that callback asked rank 1 to serve;
+      * rank 0 launches step s only once rank 1 has announced it and has not stopped since;
+      * rank 1 launches step s only after rank 0 has published its launch (launched0).
+    Rank 0 raises nothing between its launch and that publication: a launch call that fails has launched nothing, and
+    SIGINT is held back (_deferred_sigint) and turned into KeyboardInterrupt at rank 0's next gate.
+
+    get_image() inside rank 0's callback is collective on a banded scale (gather_rows): rank 1 serves the gathers rank 0
+    requests while it waits for that callback to end (at its next gate or at the end of the scale).  It has launched the
+    step rank 0 is reporting and launches nothing more until rank 0 does, so its rows are that step's."""
+
+    def __init__(self):
+        self.cond = threading.Condition()
+        self.ready1 = self.launched0 = self.done0 = 0
+        self.requested = self.served = 0
+        self.stopped = False
+        self.interrupt = None    # (handler, signum) of a SIGINT held back until rank 0's next gate
+
+    def deliver_interrupt(self):
+        """Rank 0: run the SIGINT handler held back since the signal arrived (it raises KeyboardInterrupt)."""
+        if self.interrupt is not None:
+            handler, signum = self.interrupt
+            self.interrupt = None
+            handler(signum, None)
+
+    def stop(self):
+        with self.cond:
+            self.stopped = True
+            self.cond.notify_all()
+
+    def _set(self, **kw):
+        with self.cond:
+            for k, v in kw.items():
+                setattr(self, k, v)
+            self.cond.notify_all()
+
+    def request_gather(self):
+        with self.cond:
+            self.requested += 1
+            self.cond.notify_all()
+
+    def _serve_until(self, st, done):
+        """Rank 1: serve rank 0's gathers until done() (checked first) or the stop."""
+        with self.cond:
+            while not done():
+                if self.served < self.requested:
+                    self.served += 1
+                    self.cond.release()
+                    try:
+                        st.get_image_tensor()
+                    finally:
+                        self.cond.acquire()
+                elif self.stopped:
+                    raise _Stopped()
+                else:
+                    self.cond.wait()
+
+    def before_launch(self, st, step):
+        if st._rank == 0:
+            with self.cond:
+                while True:
+                    self.deliver_interrupt()
+                    if self.stopped:
+                        raise _Stopped()
+                    if self.ready1 >= step:
+                        return
+                    self.cond.wait(0.05)    # a held-back SIGINT does not notify
+        else:
+            self._serve_until(st, lambda: self.done0 >= step - 1)
+            self._set(ready1=step)
+            with self.cond:
+                while self.launched0 < step:
+                    if self.stopped:
+                        raise _Stopped()
+                    self.cond.wait()
+
+    def after_launch(self, st, step):
+        if st._rank == 0:
+            self._set(launched0=step)
+
+    def after_iteration(self, st, step):
+        if st._rank == 0:
+            self._set(done0=step)
+
+    def end_of_scale(self, st, step):
+        if st._rank != 0:
+            self._serve_until(st, lambda: self.done0 >= step)
+
+
+@contextlib.contextmanager
+def _deferred_sigint(sync):
+    """While a two-device stylize() runs on the main thread, SIGINT only records itself; rank 0 runs the handler at its
+    next launch gate (_Lockstep.deliver_interrupt).  A KeyboardInterrupt raised wherever the signal lands could fall
+    between rank 0's launch and its publication, and rank 1 would stop one launch short of it."""
+    prev = signal.getsignal(signal.SIGINT)
+    install = threading.current_thread() is threading.main_thread() and callable(prev)
+    if install:
+        def hold(signum, frame):
+            sync.interrupt = (prev, signum)
+        signal.signal(signal.SIGINT, hold)
+    try:
+        yield
+    finally:
+        if install:
+            signal.signal(signal.SIGINT, prev)
+
+
 class StyleTransfer:
     RING_SLOTS = 8
 
@@ -323,9 +447,16 @@ class StyleTransfer:
                           f'devices={[str(d) for d in self.devices]} -> using cuda:{torch.cuda.current_device()} '
                           '(there is no CPU fallback)')
             self.devices = [torch.device('cuda', torch.cuda.current_device())]
+        # two devices in one process (ST:326-333): one rank per listed device, the large scales tiled across them as
+        # under torchrun.  An explicit group, or a torch.distributed job (one process per GPU already), keeps one
+        # device per process.
+        shared = None
         if len(self.devices) == 2:
-            warnings.warn('the reference\'s 2-device layer split (ST:326-333) is superseded; running on '
-                          f'{self.devices[0]} only')
+            if distributed is None and D.default_group() is None:
+                shared = D.ThreadGroup.Shared(2)
+            else:
+                warnings.warn('the reference\'s 2-device layer split (ST:326-333) is superseded; running on '
+                              f'{self.devices[0]} only')
         dev = self.devices[0]
         if dev.index is None:
             dev = torch.device('cuda', torch.cuda.current_device())
@@ -347,7 +478,9 @@ class StyleTransfer:
         # one process per GPU under torch.distributed: large scales are tiled spatially over the ranks.
         # `distributed`: None = the torch.distributed default group if initialised, False = never tile, or a group
         # object (distributed.TorchGroup / ThreadGroup).
-        if distributed is None or distributed is True:
+        if shared is not None:
+            self._group = D.ThreadGroup(shared, 0)
+        elif distributed is None or distributed is True:
             self._group = D.default_group()
         elif distributed is False:
             self._group = None
@@ -367,12 +500,23 @@ class StyleTransfer:
         self._comm_cap = None
         self._shared_cap = 0
         self._band = None
+        self._verbose = True
+        self._sync = None    # _Lockstep of the in-process ranks while stylize() runs
+        # rank 1 of StyleTransfer(devices=[a, b]): the same single-device machinery on the second device, driven by
+        # stylize() on a thread of its own
+        self._peer = None
+        if shared is not None:
+            self._peer = StyleTransfer([self.devices[1]], pooling, vgg_weights=vgg_weights,
+                                       distributed=D.ThreadGroup(shared, 1))
+            self._peer._verbose = False
 
     # ------------------------------------------------------------------ results
     def get_image_tensor(self):
         self._stream.synchronize()   # iterations run on the library's stream; the EMA must be complete before it is read
         value = self.average.get().detach()
         if self._band is not None:   # tiled scale in flight: the average holds this rank's rows only (collective call)
+            if self._sync is not None and self._rank == 0:
+                self._sync.request_gather()   # the in-process rank 1 joins the gather (_Lockstep)
             value = D.gather_rows(value, self._band, self._group)
         return value[0].clamp(0, 1)
 
@@ -471,6 +615,8 @@ class StyleTransfer:
                 ok = False
             if all(g.all_gather_object(ok)):
                 self._comm_cap = (cap_h, cap_w)
+            elif self._sync is not None:    # in-process ranks have no NCCL: the driver runs the job untiled
+                raise _PeerUnavailable(err)
             else:
                 warnings.warn(f'peer-memory exchange unavailable on some rank ({err}); falling back to host-driven '
                               'NCCL exchanges')
@@ -591,6 +737,114 @@ class StyleTransfer:
                 style_scale_fac: float = 1.,
                 style_size: int = None,
                 callback=None):
+        """ST:349-493.  With two devices (StyleTransfer(devices=[a, b])) the second rank runs on a thread of its own
+        for the duration of the call, during which cyclic garbage collection is switched off (gc.disable) and, on the
+        main thread, Ctrl-C takes effect at the next iteration boundary rather than at once."""
+        kw = dict(style_weights=style_weights, content_weight=content_weight, tv_weight=tv_weight,
+                  optimizer=optimizer, min_scale=min_scale, end_scale=end_scale, iterations=iterations,
+                  initial_iterations=initial_iterations, step_size=step_size, avg_decay=avg_decay, init=init,
+                  style_scale_fac=style_scale_fac, style_size=style_size)
+        if self._peer is not None:
+            return self._stylize_devices(content_image, style_images, callback, kw)
+        return self._stylize(content_image, style_images, callback=callback, **kw)
+
+    def _stylize_devices(self, content_image, style_images, callback, kw):
+        """stylize() of StyleTransfer(devices=[a, b]): rank 0 runs on the caller's thread (the user's callback runs
+        there, with the whole image), rank 1 (self._peer) on a thread of its own; both run _stylize in lockstep
+        (_Lockstep).  The first error of either rank stops both and is raised here, after rank 1's thread is joined and
+        the whole image of the stopped iteration is back in self.average."""
+        peer, shared = self._peer, self._group.shared
+        if self._dev != peer._dev and not torch.cuda.can_device_access_peer(self._dev, peer._dev):
+            return self._stylize_untiled(f'{self._dev} cannot access {peer._dev} peer to peer', content_image,
+                                         style_images, callback, kw)
+        sync = _Lockstep()
+        errors, lock = [], threading.Lock()
+
+        def fail(e):
+            with lock:
+                errors.append(e)
+            sync.stop()
+            shared.bar.abort()    # releases a rank waiting in a per-scale collective
+
+        def rank1():
+            try:
+                torch.cuda.set_device(peer._dev)
+                # no callback: rank 1's loss is read by nobody (the images do not depend on it)
+                peer._stylize(content_image, style_images, callback=None, **kw)
+            except BaseException as e:  # noqa: BLE001 -- re-raised on the caller's thread
+                fail(e)
+
+        result = None
+        thread = threading.Thread(target=rank1, name='stb-rank1')
+        gc_enabled = gc.isenabled()
+        with _deferred_sigint(sync):
+            try:
+                shared.bar.reset()
+                self._sync = peer._sync = sync
+                # no cyclic garbage collection while the ranks run: a finalizer that frees device memory synchronises
+                # the device, and run on one rank's thread while an iteration of the other waits for this rank it
+                # would stall both
+                gc.collect()
+                gc.disable()
+                thread.start()
+                result = self._stylize(content_image, style_images, callback=callback, **kw)
+            except BaseException as e:  # noqa: BLE001 -- re-raised below, once rank 1 has stopped
+                fail(e)
+            finally:
+                if thread.ident is not None:
+                    thread.join()
+                self._sync = peer._sync = None
+                if gc_enabled:
+                    gc.enable()
+            if errors:
+                try:
+                    self._stitch_stopped_bands()
+                except BaseException as e:  # noqa: BLE001 -- the first error is the one to report
+                    errors.append(e)
+            else:
+                sync.deliver_interrupt()    # a SIGINT that came after rank 0's last gate
+        if errors and isinstance(errors[0], _PeerUnavailable):
+            return self._stylize_untiled(str(errors[0]), content_image, style_images, callback, kw)
+        if errors:
+            raise errors[0]
+        return result
+
+    def _stitch_stopped_bands(self):
+        """After a two-device run stopped on a banded scale: rank 0's EMA becomes the whole image again, rank 1's own
+        rows copied in directly.  Both threads have returned and both streams are drained, so nothing changes those rows
+        any more, and both ranks launched the same iterations, so they are of the same step as rank 0's."""
+        peer, band, pband = self._peer, self._band, self._peer._band
+        self._band = peer._band = None
+        if band is None:
+            return
+        with torch.cuda.device(self._dev):
+            self._stream.synchronize()
+            peer._stream.synchronize()
+            self.model.set_band(False)
+            if pband is None or pband.H != band.H:   # rank 1 stopped before it held rows of this scale
+                self.average = None
+                return
+            own = [self.average.value[:, :, band.own0:band.own0 + band.own_rows],
+                   peer.average.value[:, :, pband.own0:pband.own0 + pband.own_rows].to(self._dev)]
+            self.average = EMA.from_state(torch.cat(own, dim=2), self.average.accum, self.average.decay)
+            self.image = self.average.get()
+
+    def _stylize_untiled(self, why, content_image, style_images, callback, kw):
+        """The job on the first device alone, rank 1 idle: the in-process ranks cannot map each other's memory, and they
+        have no NCCL to fall back on.  When the mapping failed only at the first banded scale, the job restarts: the
+        callback sees the iterations of the smaller scales again."""
+        warnings.warn(f'peer-memory exchange between {self._dev} and {self._peer._dev} unavailable ({why}); '
+                      f'running untiled on {self._dev}')
+        group = self._group
+        self._group, self._dist, self._world = None, False, 1
+        try:
+            return self._stylize(content_image, style_images, callback=callback, **kw)
+        finally:
+            self._group, self._dist, self._world = group, True, 2
+
+    def _stylize(self, content_image, style_images, *, style_weights, content_weight, tv_weight, optimizer, min_scale,
+                 end_scale, iterations, initial_iterations, step_size, avg_decay, init, style_scale_fac, style_size,
+                 callback):
         dev = self._dev
         min_scale = min(min_scale, end_scale)
         if style_weights is None:
@@ -672,12 +926,15 @@ class StyleTransfer:
                     self.image = D.local_slice(full_image, band)
                     content = D.local_slice(content, band)
                 self.average = EMA(self.image, avg_decay)
+                self._band = band   # from here on the average holds the band's rows only
 
-                print(f'Processing content image ({cw}x{ch})...')
+                if self._verbose:
+                    print(f'Processing content image ({cw}x{ch})...')
                 content_target = self.model.content_features(content)
                 means = srms = None
                 for weight, (sw, sh, simg) in zip(style_weights, styles):
-                    print(f'Processing style image ({sw}x{sh})...')
+                    if self._verbose:
+                        print(f'Processing style image ({sw}x{sh})...')
                     m_i, s_i = self._style_stats(simg, sh, sw)
                     if means is None:
                         means = [m * weight for m in m_i]
@@ -693,7 +950,6 @@ class StyleTransfer:
                                        tv_weight)
                 if band is not None:
                     self._setup_comm(band, cw)
-                    self._band = band
 
                 if optimizer == 'adam':
                     if exp_avg is None:
@@ -715,7 +971,10 @@ class StyleTransfer:
                 torch.cuda.empty_cache()
 
                 actual_its = initial_iterations if scale == scales[0] else iterations
+                sync = self._sync
                 for i in range(1, actual_its + 1):
+                    if sync is not None:
+                        sync.before_launch(self, step + 1)
                     if optimizer == 'adam' and band is not None:
                         step += 1
                         self._iterate_banded(band, stats, grad, exp_avg, exp_avg_sq, step, step_size, avg_decay)
@@ -728,6 +987,8 @@ class StyleTransfer:
                     else:
                         step += 1
                         self._iterate_lbfgs(lbfgs_state, step, avg_decay)
+                    if sync is not None:
+                        sync.after_launch(self, step)
                     if callback is not None:
                         # host-side bookkeeping first: it overlaps the iteration still running on the device (the
                         # native path allocates nothing, so the high-water mark cannot move before the sync)
@@ -743,12 +1004,16 @@ class StyleTransfer:
                         loss_value = float(self.last_loss_terms[0])
                         callback(STIterate(w=cw, h=ch, i=i, i_max=actual_its, loss=loss_value, time=time.time(),
                                            gpu_ram=gpu_ram))
+                    if sync is not None:
+                        sync.after_iteration(self, step)
+                if sync is not None:
+                    sync.end_of_scale(self, step)
 
                 if band is not None:  # stitch the bands back together (identical full tensors on every rank)
-                    self._band = None
                     g = self._group
                     self.average = EMA.from_state(D.gather_rows(self.average.value, band, g), self.average.accum,
                                                   avg_decay)
+                    self._band = None
                     if optimizer == 'adam':   # L-BFGS starts afresh every scale: it has no state to carry
                         exp_avg, exp_avg_sq = D.gather_rows(exp_avg, band, g), D.gather_rows(exp_avg_sq, band, g)
                     self.image = self.average.get()
