@@ -109,7 +109,9 @@ STB_API int stb_iterate_lbfgs(stb_ctx* ctx, float* img, float* ema, void* state,
 /* ------------------------------------------------------------------ spatial tiling across GPUs (SURVEY.md 8e)
  * A context may work on a horizontal band (plus halo aprons) of a taller image: H passed to the other calls is the
  * LOCAL height, rows [own_row0, own_row0+own_rows) (multiples of 16) are the band's own rows, H_global the full
- * height.  Only own rows enter the statistics, losses and tap gradients.  Per iteration the host runs
+ * height.  Only own rows enter the statistics, losses and tap gradients.  An iteration of a band is one call of
+ * stb_iterate_banded (or stb_iterate_lbfgs_banded), with the exchanges between the ranks inside it (below).  Where the
+ * ranks cannot map each other's memory, the host drives the same iteration in phases instead:
  *   stb_iterate_fwd  -> all-reduce(sum) of the stats block over the ranks (one NCCL call, ~2.4 MB)
  *   stb_iterate_bwd  -> grad_out = d loss / d (local image) incl. contributions to the halo rows
  *   [exchange + add the halo rows of grad_out with the neighbouring bands]
@@ -184,8 +186,8 @@ STB_API int stb_iterate_lbfgs_banded(stb_ctx* ctx, float* img, float* ema, void*
 /* 1: iterations replay as CUDA graphs, 2: enabled but nothing captured yet, 0: eager launches (note_out says why). */
 STB_API int stb_graph_status(stb_ctx* ctx, char* note_out, size_t note_bytes);
 /* Kernel launches issued through graph replays so far, counted from the captured graphs: number of replays, kernels
- * they launched (stb_iterate_lbfgs' replays included), kernel nodes per graph slot {stb_iterate, stb_iterate_fwd,
- * stb_iterate_bwd, stb_iterate_banded}. */
+ * they launched (the L-BFGS entry points' replays included), and the kernel nodes of the graphs of
+ * {stb_iterate, stb_iterate_fwd, stb_iterate_bwd, stb_iterate_banded}; the L-BFGS graphs have no entry there. */
 STB_API int stb_launch_count(stb_ctx* ctx, int64_t* graph_replays, int64_t* kernels_replayed, int* kernels_per_graph4);
 
 /* ------------------------------------------------------------------ measurement (bench.py roofline leg)

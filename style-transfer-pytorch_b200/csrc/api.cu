@@ -71,6 +71,10 @@ struct Prof {
   }
 };
 
+// one captured graph per iteration entry point; stb_launch_count reports the first four
+enum GraphSlotId { GS_ITERATE = 0, GS_ITERATE_FWD, GS_ITERATE_BWD, GS_ITERATE_BANDED, GS_ITERATE_LBFGS,
+                   GS_ITERATE_LBFGS_BANDED, GS_COUNT };
+
 struct stb_ctx {
   Prof prof;
   int device = 0;
@@ -98,9 +102,11 @@ struct stb_ctx {
   AdamScalars* d_adam = nullptr;
   long long* d_step = nullptr;
   long long dev_step_mirror = -1;  // host's view of *d_step
-  // CUDA graph of one fused iteration, keyed by everything baked into the launches
+  // CUDA graph of one fused iteration, keyed by everything baked into the launches (null / 0: not an argument of the
+  // entry point)
   struct GraphKey {
-    int H, W; const void *ws, *img, *m, *v, *ema, *loss; float lr, b1, b2, eps, decay;
+    int H, W; const void *ws, *img, *exp_avg, *exp_avg_sq, *ema, *grad_out, *state, *loss;
+    float lr, b1, b2, eps, decay;
     bool operator==(const GraphKey& o) const { return std::memcmp(this, &o, sizeof(GraphKey)) == 0; }
   };
   struct GraphSlot {
@@ -113,9 +119,7 @@ struct stb_ctx {
       exec = nullptr; key = GraphKey{}; hits = 0; kernel_nodes = 0;
     }
   };
-  // 0: stb_iterate, 1: stb_iterate_fwd, 2: stb_iterate_bwd (host-driven phases), 3: stb_iterate_banded,
-  // 4: stb_iterate_lbfgs, 5: stb_iterate_lbfgs_banded
-  GraphSlot gslot[6];
+  GraphSlot gslot[GS_COUNT];
   void reset_graphs() { for (auto& g : gslot) g.reset(); }
   bool graphs_enabled = true;
   std::string graph_note;  // why graph replay was switched off for this context (stb_graph_status)
@@ -206,20 +210,24 @@ int ensure_ws(const stb_ctx* ctx, const Plan& pl) {
 template <typename T>
 T* at(const stb_ctx* ctx, size_t off) { return reinterpret_cast<T*>(ctx->ws + off); }
 
-struct BandRows { int own0, rows, h_global; };
-// own rows of conv i's output grid (level = number of pools before it) and the global height at that level
-BandRows band_rows(const stb_ctx* ctx, const Plan& pl, int conv) {
+// pyramid level of conv i's grid: the number of pools before it
+int level_of(int conv) {
   int level = 0;
   for (int i = 0; i < conv; ++i)
     if (kPoolAfter[i]) ++level;
+  return level;
+}
+
+struct BandRows { int own0, rows, h_global; };
+// own rows of conv i's output grid and the global height at its level
+BandRows band_rows(const stb_ctx* ctx, const Plan& pl, int conv) {
   BandRows b;
   if (!ctx->band_on) { b.own0 = 0; b.rows = pl.h[conv]; b.h_global = pl.h[conv]; return b; }
+  const int level = level_of(conv);
   const bool is_bottom = ctx->band_own0 + ctx->band_own_rows >= pl.H;
   b.own0 = ctx->band_own0 >> level;
   b.rows = is_bottom ? pl.h[conv] - b.own0 : (ctx->band_own_rows >> level);
-  int hg = ctx->band_H_global;
-  for (int i = 0; i < level; ++i) hg /= 2;
-  b.h_global = hg;
+  b.h_global = ctx->band_H_global >> level;   // floor-mode pools of a positive height
   return b;
 }
 
@@ -227,12 +235,6 @@ BandRows band_rows(const stb_ctx* ctx, const Plan& pl, int conv) {
 // rows of every activation / gradient tensor; the row above and the row below them, which the next 3x3 kernel reads,
 // are the neighbours' boundary own rows and are pulled straight out of the neighbours' workspaces.
 struct HaloPlans { Plan up, dn; };
-int level_of(int conv) {
-  int level = 0;
-  for (int i = 0; i < conv; ++i)
-    if (kPoolAfter[i]) ++level;
-  return level;
-}
 // tensor with C channels at pyramid level `level` (width w_l); off_* = its byte offset in the plan of me / up / down.
 // sync_only: publish + wait the stamps without copying (a buffer the neighbours pulled from is about to be rewritten).
 int halo_exchange(stb_ctx* ctx, int level, int w_l, int C, size_t off_me, size_t off_up, size_t off_dn,
@@ -346,12 +348,7 @@ __global__ void adam_rows_kernel(float* __restrict__ img, const float* __restric
     const size_t idx = ((size_t)c * H + row0) * W + r;
     const float g = grad[idx];
     float m = exp_avg[idx], v = exp_avg_sq[idx], p = img[idx], e = ema[idx];
-    m = m + (g - m) * ac.one_minus_b1;
-    v = v * ac.b2 + ac.one_minus_b2 * g * g;
-    const float denom = sqrtf(v) * ac.inv_sqrt_bc2 + ac.eps;
-    p = p - ac.step_size * (m / denom);
-    p = fminf(fmaxf(p, 0.f), 1.f);
-    e = e * ac.ema_decay + ac.one_minus_decay * p;
+    adam_element(ac, g, m, v, p, e);
     exp_avg[idx] = m; exp_avg_sq[idx] = v; img[idx] = p; ema[idx] = e;
   }
 }
@@ -362,14 +359,7 @@ __global__ void adam_scalars_kernel(long long* step, AdamScalars* out, float lr,
                                     float adam_eps, float ema_decay) {
   const long long t = *step + 1;
   *step = t;
-  const double bc1 = 1.0 - pow((double)beta1, (double)t);
-  const double bc2 = 1.0 - pow((double)beta2, (double)t);
-  AdamScalars as;
-  as.one_minus_b1 = 1.f - beta1; as.b2 = beta2; as.one_minus_b2 = 1.f - beta2;
-  as.step_size = (float)((double)lr / bc1);
-  as.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
-  as.eps = adam_eps; as.ema_decay = ema_decay; as.one_minus_decay = 1.f - ema_decay;
-  *out = as;
+  *out = make_adam_scalars(t, lr, beta1, beta2, adam_eps, ema_decay);
 }
 
 // the iteration counter of the loss ring's stamps on a path without Adam scalars (stb_iterate_lbfgs)
@@ -408,20 +398,6 @@ __global__ void finalize_loss_kernel(const float* __restrict__ scalars, float co
   }
 }
 
-}  // namespace
-
-AdamScalars stb::make_adam_scalars(int64_t step, float lr, float beta1, float beta2, float adam_eps, float ema_decay) {
-  AdamScalars as{};
-  const double bc1 = 1.0 - std::pow((double)beta1, (double)step);
-  const double bc2 = 1.0 - std::pow((double)beta2, (double)step);
-  as.one_minus_b1 = 1.f - beta1; as.b2 = beta2; as.one_minus_b2 = 1.f - beta2;
-  as.step_size = (float)((double)lr / bc1);
-  as.inv_sqrt_bc2 = (float)(1.0 / std::sqrt(bc2));
-  as.eps = adam_eps; as.ema_decay = ema_decay; as.one_minus_decay = 1.f - ema_decay;
-  return as;
-}
-
-namespace {
 void comm_release(stb_ctx* ctx) {
   if (ctx->comm_ipc)
     for (int r = 0; r < ctx->comm.world; ++r)
@@ -631,7 +607,7 @@ int stb_set_targets(stb_ctx* ctx, int H, int W, const void* content_target_bf16,
 namespace {
 
 // phase 1: forward + this context's (band-local) statistics into the stats block
-int iterate_fwd(stb_ctx* ctx, const Plan& pl, const float* img, cudaStream_t s, const HaloPlans* halo = nullptr) {
+int iterate_fwd(stb_ctx* ctx, const Plan& pl, const float* img, cudaStream_t s, const HaloPlans* halo) {
   STB_TRY(forward(ctx, pl, img, NCONV - 1, true, s, halo));
   STB_TRY(style_grams(ctx, pl, s));
   const BandRows b22 = band_rows(ctx, pl, kContentConv);
@@ -648,10 +624,13 @@ int iterate_fwd(stb_ctx* ctx, const Plan& pl, const float* img, cudaStream_t s, 
   return STB_OK;
 }
 
-// phase 2: W2 losses on the (globally reduced) statistics, backward to the image, optional fused update
-int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, float* exp_avg, float* exp_avg_sq, float* ema,
-                const AdamScalars* d_adam, int apply_update, float* grad_out, float* loss_out_host8, cudaStream_t s,
-                const HaloPlans* halo = nullptr, bool publish_loss = false) {
+// Adam + clamp + EMA fused into the epilogue of conv0's dgrad (d_adam: the device scalars of this step)
+struct FusedAdam { float *exp_avg, *exp_avg_sq, *ema; const AdamScalars* d_adam; };
+
+// phase 2: W2 losses on the (globally reduced) statistics, backward to the image, optional fused update.
+// publish_loss: the loss kernel also writes the loss ring (stb_set_loss_ring) under the device step counter.
+int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, const FusedAdam* update, bool publish_loss, float* grad_out,
+                float* loss_out_host8, cudaStream_t s, const HaloPlans* halo) {
   const int H = pl.H, W = pl.W;
   const long n22 = (long)band_rows(ctx, pl, kContentConv).h_global * pl.w[kContentConv] * 512;  // global numel
   float* loss_dev = at<float>(ctx, pl.loss_off);
@@ -663,9 +642,7 @@ int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, float* exp_avg, float*
   ctx->prof.begin(PC_FINALIZE, s);
   finalize_loss_kernel<<<1, 32, 0, s>>>(at<float>(ctx, pl.stats_off) + pl.stats_scalars,
                                         ctx->content_weight / (float)n22, loss_dev + 16, ctx->tv_weight, loss_dev,
-                                        apply_update || ctx->band_on || publish_loss ? ctx->ring_dev : nullptr,
-                                        ctx->ring_slots,
-                                        ctx->d_step);
+                                        publish_loss ? ctx->ring_dev : nullptr, ctx->ring_slots, ctx->d_step);
   ctx->prof.end(s);
   if (loss_out_host8)
     STB_CUDA_CHECK(cudaMemcpyAsync(loss_out_host8, loss_dev, 8 * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -749,11 +726,12 @@ int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, float* exp_avg, float*
   }
   // conv0 backward: interior pixels on the tensor cores (1x1 GEMM + col2im) with the optimiser step as epilogue;
   // the border pixels (adjoint of the replicate pad) and their update in SIMT
+  const FusedAdam u = update ? *update : FusedAdam{};
   ctx->prof.begin(PC_CONV0_BWD_ADAM, s);
-  STB_TRY(launch_conv0_bwd_interior(g[cur], ctx->wb[0], at<float>(ctx, pl.gtv_off), img, exp_avg, exp_avg_sq, ema,
-                                    grad_out, H, W, d_adam, apply_update, s));
-  STB_TRY(launch_conv0_bwd_adam(g[cur], true, ctx->w0, at<float>(ctx, pl.gtv_off), img, exp_avg, exp_avg_sq, ema,
-                                grad_out, H, W, d_adam, apply_update, s));
+  STB_TRY(launch_conv0_bwd_interior(g[cur], ctx->wb[0], at<float>(ctx, pl.gtv_off), img, u.exp_avg, u.exp_avg_sq,
+                                    u.ema, grad_out, H, W, u.d_adam, update != nullptr, s));
+  STB_TRY(launch_conv0_bwd_adam(g[cur], true, ctx->w0, at<float>(ctx, pl.gtv_off), img, u.exp_avg, u.exp_avg_sq, u.ema,
+                                grad_out, H, W, u.d_adam, update != nullptr, s));
   ctx->prof.end(s);
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
@@ -765,7 +743,7 @@ int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, float* exp_avg, float*
 // a captured graph removes the per-launch host cost and the tensor-map encodes (matters most at the small pyramid
 // levels and when the image is tiled over many GPUs).  `key` holds everything that is baked into the launches.
 template <typename Run>
-int run_graphed(stb_ctx* ctx, int slot, const stb_ctx::GraphKey& key, bool allowed, cudaStream_t s, Run&& run) {
+int run_graphed(stb_ctx* ctx, GraphSlotId slot, const stb_ctx::GraphKey& key, bool allowed, cudaStream_t s, Run&& run) {
   const bool legacy = (s == nullptr || s == cudaStreamLegacy || s == cudaStreamPerThread);
   if (!ctx->graphs_enabled || ctx->prof.on || legacy || !allowed) return run();
   stb_ctx::GraphSlot& g = ctx->gslot[slot];
@@ -820,6 +798,152 @@ namespace stb {
 const CommDev* ctx_comm(const stb_ctx* ctx) { return ctx->comm_ready && ctx->comm_geometry ? &ctx->comm : nullptr; }
 }  // namespace stb
 
+// ---- the iteration entry points.  Each records one variant of the launch sequence
+//   [comm phase 0 + halo pull] -> forward + statistics -> [all-reduce of the statistics] -> step kernel ->
+//   W2 + backward -> [comm phase 2 -> update -> comm phase 3]
+// (brackets: a band's iteration with the exchanges inside, comm.cu), or the untiled L-BFGS step after the backward.
+namespace {
+
+enum StepKernel { STEP_NONE, STEP_ADAM_SCALARS, STEP_ADVANCE };   // both advance the device step counter
+enum Update { UPDATE_NONE, UPDATE_ADAM_FUSED, UPDATE_ADAM_SEAM, UPDATE_LBFGS, UPDATE_LBFGS_BANDED };
+struct Variant {
+  const char* name;   // the entry point, for the error texts
+  GraphSlotId slot;
+  bool fwd, bwd;      // records the forward / the backward half (the host-driven phases of a band record one each)
+  bool banded;
+  StepKernel step;
+  Update update;      // ADAM_FUSED: in the epilogue of conv0's dgrad; ADAM_SEAM / LBFGS_BANDED: after the seam exchange
+};
+constexpr Variant kIterate{"stb_iterate", GS_ITERATE, true, true, false, STEP_ADAM_SCALARS, UPDATE_ADAM_FUSED};
+constexpr Variant kClosure{"stb_iterate", GS_ITERATE, true, true, false, STEP_NONE, UPDATE_NONE};   // never graphed
+constexpr Variant kFwd{"stb_iterate_fwd", GS_ITERATE_FWD, true, false, false, STEP_NONE, UPDATE_NONE};
+constexpr Variant kBwd{"stb_iterate_bwd", GS_ITERATE_BWD, false, true, false, STEP_NONE, UPDATE_NONE};
+constexpr Variant kLbfgs{"stb_iterate_lbfgs", GS_ITERATE_LBFGS, true, true, false, STEP_ADVANCE, UPDATE_LBFGS};
+constexpr Variant kBanded{"stb_iterate_banded", GS_ITERATE_BANDED, true, true, true, STEP_ADAM_SCALARS,
+                          UPDATE_ADAM_SEAM};
+constexpr Variant kLbfgsBanded{"stb_iterate_lbfgs_banded", GS_ITERATE_LBFGS_BANDED, true, true, true, STEP_ADVANCE,
+                               UPDATE_LBFGS_BANDED};
+
+// the caller's arguments in the order of the C ABI (null / 0 where the entry point has no such argument)
+struct IterArgs {
+  float *img, *exp_avg, *exp_avg_sq, *ema;
+  int64_t step;
+  float lr, beta1, beta2, adam_eps, ema_decay;
+  float *grad_out, *loss_out_host8;
+  void* state;   // L-BFGS
+  size_t state_bytes;
+};
+
+// the optimizer state the update reads; a band's L-BFGS state holds its own rows
+int check_optimizer_state(const stb_ctx* ctx, const Variant& v, const IterArgs& a) {
+  if (v.update == UPDATE_ADAM_FUSED || v.update == UPDATE_ADAM_SEAM)
+    STB_CHECK(a.exp_avg && a.exp_avg_sq && a.ema && a.step >= 1, STB_ERR_INVALID, "bad optimizer state");
+  if (v.update == UPDATE_LBFGS || v.update == UPDATE_LBFGS_BANDED) {
+    STB_CHECK(a.step >= 1, STB_ERR_INVALID, "step must be >= 1");
+    STB_CHECK((reinterpret_cast<uintptr_t>(a.state) & 255) == 0 && (reinterpret_cast<uintptr_t>(a.img) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(a.ema) & 15) == 0,
+              STB_ERR_INVALID, "state must be 256-byte aligned, img and ema 16-byte aligned");
+    const int rows = v.banded ? ctx->band_own_rows : ctx->tH;
+    const size_t need = lbfgs_state_bytes(3l * rows * ctx->tW);
+    STB_CHECK(a.state_bytes >= need, STB_ERR_INVALID,
+              "L-BFGS state of %zu bytes is too small for %d rows x %d (needs %zu)", a.state_bytes, rows, ctx->tW, need);
+  }
+  return STB_OK;
+}
+
+// state, workspace and argument checks of an entry point, before anything is launched
+int check_iteration(stb_ctx* ctx, const Variant& v, const IterArgs& a, Plan* pl) {
+  if (v.banded) {
+    STB_CHECK(ctx->targets_set && ctx->band_on, STB_ERR_STATE, "stb_set_band + stb_set_targets must precede %s",
+              v.name);
+    STB_CHECK(ctx->comm_ready && ctx->comm_geometry, STB_ERR_STATE, "stb_comm_connect_* + stb_comm_set_geometry first");
+  } else {
+    STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede %s", v.name);
+    STB_CHECK(v.update == UPDATE_NONE || !ctx->band_on, STB_ERR_STATE,
+              "%s updates the whole image but the context has a band set (stb_iterate_banded / "
+              "stb_iterate_lbfgs_banded iterate a band)", v.name);
+    STB_TRY(check_optimizer_state(ctx, v, a));
+  }
+  make_plan(ctx, ctx->tH, ctx->tW, pl);
+  STB_TRY(ensure_ws(ctx, *pl));
+  if (!v.banded) return STB_OK;
+  const CommDev& c = ctx->comm;
+  STB_CHECK(c.h_local == pl->H && c.W == pl->W && c.own0 == ctx->band_own0 && c.own_rows == ctx->band_own_rows,
+            STB_ERR_STATE, "comm geometry (%dx%d, own %d+%d) does not match the band (%dx%d, own %d+%d)", c.h_local,
+            c.W, c.own0, c.own_rows, pl->H, pl->W, ctx->band_own0, ctx->band_own_rows);
+  STB_TRY(check_optimizer_state(ctx, v, a));
+  STB_CHECK(!ctx->halo_mode || (ctx->ws == ctx->shared_ws && ctx->shared_ws != nullptr), STB_ERR_STATE,
+            "halo mode needs the library-owned workspace bound (stb_comm_alloc_workspace)");
+  return STB_OK;
+}
+
+// graphable = false: eager launches, the graph slot is left alone
+int iterate(stb_ctx* ctx, const Variant& v, const IterArgs& a, bool graphable, void* stream) {
+  STB_ENTER(ctx);
+  Plan pl;
+  STB_TRY(check_iteration(ctx, v, a, &pl));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (v.step != STEP_NONE) {
+    // the device step counter must read step-1 before this iteration (it is carried across scales like ST:461-462)
+    if (ctx->dev_step_mirror != a.step - 1) {
+      const long long prev = a.step - 1;
+      STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &prev, sizeof(prev), cudaMemcpyHostToDevice, s));
+      STB_CUDA_CHECK(cudaStreamSynchronize(s));  // `prev` is a stack variable; this path runs once per scale at most
+    }
+    ctx->dev_step_mirror = a.step;
+  }
+  const CommDev& c = ctx->comm;
+  HaloPlans hp;
+  const HaloPlans* halo = nullptr;
+  if (v.banded && ctx->halo_mode) {
+    // per-layer-halo mode: the neighbours' buffers sit at the offsets of THEIR plans (edge bands have one apron less)
+    make_plan(ctx, c.rank > 0 ? c.up_h_local : pl.H, pl.W, &hp.up);
+    make_plan(ctx, c.rank + 1 < c.world ? c.dn_h_local : pl.H, pl.W, &hp.dn);
+    halo = &hp;
+  }
+  const long n = 3l * pl.H * pl.W;
+  float* grad = v.banded ? reinterpret_cast<float*>(c.mbox[c.rank] + c.off_grad)
+                : v.update == UPDATE_LBFGS ? lbfgs_grad_buffer(a.state, n) : a.grad_out;
+  const FusedAdam fused{a.exp_avg, a.exp_avg_sq, a.ema, ctx->d_adam};
+  // the loss ring's stamp is the device step counter: the calls that advance it write the ring, and so does every call
+  // on a band
+  const bool publish_loss = v.step != STEP_NONE || ctx->band_on;
+  auto run = [&]() -> int {
+    ctx->halo_seq = 0;
+    if (v.fwd) {
+      if (v.banded) {
+        STB_TRY(launch_comm_phase(c, 0, s));
+        STB_TRY(launch_halo_pull(c, a.img, s));
+      }
+      STB_TRY(iterate_fwd(ctx, pl, a.img, s, halo));
+      if (v.banded) STB_TRY(launch_stats_allreduce(c, at<float>(ctx, pl.stats_off), pl.stats_floats, s));
+    }
+    if (v.step == STEP_ADAM_SCALARS)
+      adam_scalars_kernel<<<1, 1, 0, s>>>(ctx->d_step, ctx->d_adam, a.lr, a.beta1, a.beta2, a.adam_eps, a.ema_decay);
+    else if (v.step == STEP_ADVANCE)
+      advance_step_kernel<<<1, 1, 0, s>>>(ctx->d_step);
+    if (v.bwd)
+      STB_TRY(iterate_bwd(ctx, pl, a.img, v.update == UPDATE_ADAM_FUSED ? &fused : nullptr, publish_loss, grad,
+                          a.loss_out_host8, s, halo));
+    if (v.update == UPDATE_LBFGS) return launch_lbfgs_step(a.state, n, a.img, a.ema, a.ema_decay, s);
+    if (!v.banded) return STB_OK;
+    STB_TRY(launch_comm_phase(c, 2, s));
+    if (v.update == UPDATE_ADAM_SEAM)
+      STB_TRY(launch_adam_seam(c, a.img, a.exp_avg, a.exp_avg_sq, a.ema, ctx->d_adam, halo ? 0 : 1, s));
+    else
+      STB_TRY(launch_lbfgs_step_banded(a.state, c, a.img, a.ema, a.ema_decay, halo ? 0 : 1, s));
+    return launch_comm_phase(c, 3, s);
+  };
+  stb_ctx::GraphKey key;
+  std::memset(&key, 0, sizeof(key));   // compared bytewise
+  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = a.img; key.exp_avg = a.exp_avg; key.exp_avg_sq = a.exp_avg_sq;
+  key.ema = a.ema; key.grad_out = a.grad_out; key.state = a.state; key.loss = a.loss_out_host8;
+  key.lr = a.lr; key.b1 = a.beta1; key.b2 = a.beta2; key.eps = a.adam_eps; key.decay = a.ema_decay;
+  return run_graphed(ctx, v.slot, key, graphable, s, run);
+}
+
+}  // namespace
+
 extern "C" {
 
 // One pass of ST:480-486.  apply_update = 0 evaluates loss / gradient only (test hook, L-BFGS closure).
@@ -827,39 +951,13 @@ int stb_iterate_ex(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, 
                    float beta1, float beta2, float adam_eps, float ema_decay, int apply_update, float* grad_out,
                    float* loss_out_host8, void* stream) {
   STB_CHECK(ctx && img, STB_ERR_INVALID, "null argument");
-  STB_ENTER(ctx);
-  STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede stb_iterate");
-  STB_CHECK(!(ctx->band_on && apply_update), STB_ERR_STATE,
-            "banded contexts update through stb_iterate_fwd / all-reduce / stb_iterate_bwd / stb_adam_update");
-  if (apply_update) STB_CHECK(exp_avg && exp_avg_sq && ema && step >= 1, STB_ERR_INVALID, "bad optimizer state");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  Plan pl;
-  make_plan(ctx, ctx->tH, ctx->tW, &pl);
-  STB_TRY(ensure_ws(ctx, pl));
-  if (!apply_update) {
-    STB_TRY(iterate_fwd(ctx, pl, img, s));
-    return iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad_out, loss_out_host8, s);
-  }
-  // the device step counter must read step-1 before this iteration (it is carried across scales like ST:461-462)
-  if (ctx->dev_step_mirror != step - 1) {
-    const long long v = step - 1;
-    STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &v, sizeof(v), cudaMemcpyHostToDevice, s));
-    STB_CUDA_CHECK(cudaStreamSynchronize(s));  // `v` is a stack variable; this path runs once per scale at most
-  }
-  ctx->dev_step_mirror = step;
-  auto run = [&]() -> int {
-    STB_TRY(iterate_fwd(ctx, pl, img, s));
-    adam_scalars_kernel<<<1, 1, 0, s>>>(ctx->d_step, ctx->d_adam, lr, beta1, beta2, adam_eps, ema_decay);
-    return iterate_bwd(ctx, pl, img, exp_avg, exp_avg_sq, ema, ctx->d_adam, 1, grad_out, loss_out_host8, s);
-  };
-  stb_ctx::GraphKey key{};
-  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = exp_avg; key.v = exp_avg_sq; key.ema = ema;
-  key.loss = loss_out_host8; key.lr = lr; key.b1 = beta1; key.b2 = beta2; key.eps = adam_eps; key.decay = ema_decay;
-  return run_graphed(ctx, 0, key, grad_out == nullptr, s, run);
+  const IterArgs a{img, exp_avg, exp_avg_sq, ema, step, lr, beta1, beta2, adam_eps, ema_decay, grad_out, loss_out_host8};
+  return iterate(ctx, apply_update ? kIterate : kClosure, a, apply_update && grad_out == nullptr, stream);
 }
 
-// ---- spatial tiling across GPUs (SURVEY.md section 8e): the host drives
-//   stb_iterate_fwd -> all-reduce(stats block) -> stb_iterate_bwd -> seam exchange of grad -> stb_adam_update
+// ---- spatial tiling across GPUs (SURVEY.md section 8e).  A band's iteration is stb_iterate_banded; without peer
+// memory the host drives its phases: stb_iterate_fwd -> all-reduce(stats block) -> stb_iterate_bwd -> seam exchange
+// of grad -> stb_adam_update
 int stb_set_band(stb_ctx* ctx, int enabled, int H_global, int own_row0, int own_rows) {
   STB_CHECK(ctx != nullptr, STB_ERR_INVALID, "null ctx");
   if (enabled) {
@@ -884,33 +982,18 @@ int stb_stats_block(stb_ctx* ctx, int H, int W, float** dev_ptr, size_t* n_float
 
 int stb_iterate_fwd(stb_ctx* ctx, const float* img, void* stream) {
   STB_CHECK(ctx && img, STB_ERR_INVALID, "null argument");
-  STB_ENTER(ctx);
-  STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede stb_iterate_fwd");
-  Plan pl;
-  make_plan(ctx, ctx->tH, ctx->tW, &pl);
-  STB_TRY(ensure_ws(ctx, pl));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  stb_ctx::GraphKey key{};
-  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img;
-  return run_graphed(ctx, 1, key, true, s, [&]() -> int { return iterate_fwd(ctx, pl, img, s); });
+  return iterate(ctx, kFwd, IterArgs{const_cast<float*>(img)}, true, stream);   // the forward only reads img
 }
 
 int stb_iterate_bwd(stb_ctx* ctx, float* img, float* grad_out, float* loss_out_host8, void* stream) {
   STB_CHECK(ctx && img && grad_out, STB_ERR_INVALID, "null argument");
-  STB_ENTER(ctx);
-  STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede stb_iterate_bwd");
-  Plan pl;
-  make_plan(ctx, ctx->tH, ctx->tW, &pl);
-  STB_TRY(ensure_ws(ctx, pl));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  stb_ctx::GraphKey key{};
-  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = grad_out; key.loss = loss_out_host8;
-  return run_graphed(ctx, 2, key, true, s, [&]() -> int {
-    return iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad_out, loss_out_host8, s);
-  });
+  IterArgs a{img};
+  a.grad_out = grad_out;
+  a.loss_out_host8 = loss_out_host8;
+  return iterate(ctx, kBwd, a, true, stream);
 }
 
-// Adam + clamp + EMA on rows [row0, row0+rows) of [3][H][W] fp32 tensors (the band's own rows)
+// Adam + clamp + EMA on rows [row0, row0+rows) of [3][H][W] fp32 tensors (the band's own rows, host-driven phases)
 int stb_adam_update(float* img, const float* grad, float* exp_avg, float* exp_avg_sq, float* ema, int H, int W,
                     int row0, int rows, int64_t step, float lr, float beta1, float beta2, float adam_eps,
                     float ema_decay, void* stream) {
@@ -955,39 +1038,9 @@ int stb_lbfgs_reset(void* state, int H, int W, void* stream) {
 int stb_iterate_lbfgs(stb_ctx* ctx, float* img, float* ema, void* state, size_t state_bytes, int64_t step,
                       float ema_decay, float* loss_out_host8, void* stream) {
   STB_CHECK(ctx && img && ema && state, STB_ERR_INVALID, "null argument");
-  STB_ENTER(ctx);
-  STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede stb_iterate_lbfgs");
-  STB_CHECK(!ctx->band_on, STB_ERR_STATE, "L-BFGS runs on the whole image: the context has a band set");
-  STB_CHECK(step >= 1, STB_ERR_INVALID, "step must be >= 1");
-  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0 &&
-                (reinterpret_cast<uintptr_t>(ema) & 15) == 0,
-            STB_ERR_INVALID, "state must be 256-byte aligned, img and ema 16-byte aligned");
-  const long n = 3l * ctx->tH * ctx->tW;
-  STB_CHECK(state_bytes >= lbfgs_state_bytes(n), STB_ERR_INVALID,
-            "L-BFGS state of %zu bytes is too small for %dx%d (needs %zu)", state_bytes, ctx->tH, ctx->tW,
-            lbfgs_state_bytes(n));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  Plan pl;
-  make_plan(ctx, ctx->tH, ctx->tW, &pl);
-  STB_TRY(ensure_ws(ctx, pl));
-  // the loss ring's stamp is the device step counter, carried across scales like Adam's (stb_iterate_ex)
-  if (ctx->dev_step_mirror != step - 1) {
-    const long long v = step - 1;
-    STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &v, sizeof(v), cudaMemcpyHostToDevice, s));
-    STB_CUDA_CHECK(cudaStreamSynchronize(s));  // `v` is a stack variable; this path runs once per scale at most
-  }
-  ctx->dev_step_mirror = step;
-  float* grad = lbfgs_grad_buffer(state, n);
-  auto run = [&]() -> int {
-    STB_TRY(iterate_fwd(ctx, pl, img, s));
-    advance_step_kernel<<<1, 1, 0, s>>>(ctx->d_step);
-    STB_TRY(iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad, loss_out_host8, s, nullptr, true));
-    return launch_lbfgs_step(state, n, img, ema, ema_decay, s);
-  };
-  stb_ctx::GraphKey key{};
-  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = state; key.ema = ema;
-  key.loss = loss_out_host8; key.decay = ema_decay;
-  return run_graphed(ctx, 4, key, true, s, run);
+  IterArgs a{img, nullptr, nullptr, ema, step};
+  a.ema_decay = ema_decay; a.loss_out_host8 = loss_out_host8; a.state = state; a.state_bytes = state_bytes;
+  return iterate(ctx, kLbfgs, a, true, stream);
 }
 
 // Per-kernel-class device timing (CUDA events on the launching stream).  enable: 1 starts recording spans for
@@ -1229,7 +1282,9 @@ int stb_comm_set_geometry(stb_ctx* ctx, int W, int h_local, int own0, int own_ro
             "halo-row mode needs stb_comm_alloc_workspace + stb_comm_connect_ws_*");
   ctx->halo_mode = halo_rows != 0;
   ctx->comm_geometry = true;
-  ctx->gslot[3].reset();
+  // the banded graphs bake in the halo mode and the neighbours' heights
+  ctx->gslot[GS_ITERATE_BANDED].reset();
+  ctx->gslot[GS_ITERATE_LBFGS_BANDED].reset();
   return STB_OK;
 }
 
@@ -1248,50 +1303,8 @@ int stb_iterate_banded(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_
                        float beta1, float beta2, float adam_eps, float ema_decay, float* loss_out_host8,
                        void* stream) {
   STB_CHECK(ctx && img && exp_avg && exp_avg_sq && ema && step >= 1, STB_ERR_INVALID, "bad argument");
-  STB_ENTER(ctx);
-  STB_CHECK(ctx->targets_set && ctx->band_on, STB_ERR_STATE, "stb_set_band + stb_set_targets must precede");
-  STB_CHECK(ctx->comm_ready && ctx->comm_geometry, STB_ERR_STATE, "stb_comm_connect_* + stb_comm_set_geometry first");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  Plan pl;
-  make_plan(ctx, ctx->tH, ctx->tW, &pl);
-  STB_TRY(ensure_ws(ctx, pl));
-  const CommDev& c = ctx->comm;
-  STB_CHECK(c.h_local == pl.H && c.W == pl.W && c.own0 == ctx->band_own0 && c.own_rows == ctx->band_own_rows,
-            STB_ERR_STATE, "comm geometry (%dx%d, own %d+%d) does not match the band (%dx%d, own %d+%d)", c.h_local,
-            c.W, c.own0, c.own_rows, pl.H, pl.W, ctx->band_own0, ctx->band_own_rows);
-  if (ctx->dev_step_mirror != step - 1) {
-    const long long v = step - 1;
-    STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &v, sizeof(v), cudaMemcpyHostToDevice, s));
-    STB_CUDA_CHECK(cudaStreamSynchronize(s));
-  }
-  ctx->dev_step_mirror = step;
-  float* grad = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_grad);
-  // per-layer-halo mode: the neighbours' buffers sit at the offsets of THEIR plans (edge bands have one apron less)
-  HaloPlans hp;
-  const HaloPlans* halo = nullptr;
-  if (ctx->halo_mode) {
-    STB_CHECK(ctx->ws == ctx->shared_ws && ctx->shared_ws != nullptr, STB_ERR_STATE,
-              "halo mode needs the library-owned workspace bound (stb_comm_alloc_workspace)");
-    make_plan(ctx, c.rank > 0 ? c.up_h_local : pl.H, pl.W, &hp.up);
-    make_plan(ctx, c.rank + 1 < c.world ? c.dn_h_local : pl.H, pl.W, &hp.dn);
-    halo = &hp;
-  }
-  auto run = [&]() -> int {
-    ctx->halo_seq = 0;
-    STB_TRY(launch_comm_phase(c, 0, s));
-    STB_TRY(launch_halo_pull(c, img, s));
-    STB_TRY(iterate_fwd(ctx, pl, img, s, halo));
-    STB_TRY(launch_stats_allreduce(c, at<float>(ctx, pl.stats_off), pl.stats_floats, s));
-    adam_scalars_kernel<<<1, 1, 0, s>>>(ctx->d_step, ctx->d_adam, lr, beta1, beta2, adam_eps, ema_decay);
-    STB_TRY(iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad, loss_out_host8, s, halo));
-    STB_TRY(launch_comm_phase(c, 2, s));
-    STB_TRY(launch_adam_seam(c, img, exp_avg, exp_avg_sq, ema, ctx->d_adam, halo ? 0 : 1, s));
-    return launch_comm_phase(c, 3, s);
-  };
-  stb_ctx::GraphKey key{};
-  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = exp_avg; key.v = exp_avg_sq; key.ema = ema;
-  key.loss = loss_out_host8; key.lr = lr; key.b1 = beta1; key.b2 = beta2; key.eps = adam_eps; key.decay = ema_decay;
-  return run_graphed(ctx, 3, key, true, s, run);
+  const IterArgs a{img, exp_avg, exp_avg_sq, ema, step, lr, beta1, beta2, adam_eps, ema_decay, nullptr, loss_out_host8};
+  return iterate(ctx, kBanded, a, true, stream);
 }
 
 // optimizer='lbfgs' on a band: the sequence of stb_iterate_banded up to the gradient stamp, then the banded L-BFGS step
@@ -1300,57 +1313,9 @@ int stb_iterate_banded(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_
 int stb_iterate_lbfgs_banded(stb_ctx* ctx, float* img, float* ema, void* state, size_t state_bytes, int64_t step,
                              float ema_decay, float* loss_out_host8, void* stream) {
   STB_CHECK(ctx && img && ema && state, STB_ERR_INVALID, "null argument");
-  STB_ENTER(ctx);
-  STB_CHECK(ctx->targets_set && ctx->band_on, STB_ERR_STATE, "stb_set_band + stb_set_targets must precede");
-  STB_CHECK(ctx->comm_ready && ctx->comm_geometry, STB_ERR_STATE, "stb_comm_connect_* + stb_comm_set_geometry first");
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  Plan pl;
-  make_plan(ctx, ctx->tH, ctx->tW, &pl);
-  STB_TRY(ensure_ws(ctx, pl));
-  const CommDev& c = ctx->comm;
-  STB_CHECK(c.h_local == pl.H && c.W == pl.W && c.own0 == ctx->band_own0 && c.own_rows == ctx->band_own_rows,
-            STB_ERR_STATE, "comm geometry (%dx%d, own %d+%d) does not match the band (%dx%d, own %d+%d)", c.h_local,
-            c.W, c.own0, c.own_rows, pl.H, pl.W, ctx->band_own0, ctx->band_own_rows);
-  STB_CHECK(step >= 1, STB_ERR_INVALID, "step must be >= 1");
-  STB_CHECK((reinterpret_cast<uintptr_t>(state) & 255) == 0 && (reinterpret_cast<uintptr_t>(img) & 15) == 0 &&
-                (reinterpret_cast<uintptr_t>(ema) & 15) == 0,
-            STB_ERR_INVALID, "state must be 256-byte aligned, img and ema 16-byte aligned");
-  const long n = 3l * c.own_rows * c.W;
-  STB_CHECK(state_bytes >= lbfgs_state_bytes(n), STB_ERR_INVALID,
-            "L-BFGS state of %zu bytes is too small for %d own rows x %d (needs %zu)", state_bytes, c.own_rows, c.W,
-            lbfgs_state_bytes(n));
-  if (ctx->dev_step_mirror != step - 1) {
-    const long long v = step - 1;
-    STB_CUDA_CHECK(cudaMemcpyAsync(ctx->d_step, &v, sizeof(v), cudaMemcpyHostToDevice, s));
-    STB_CUDA_CHECK(cudaStreamSynchronize(s));  // `v` is a stack variable; this path runs once per scale at most
-  }
-  ctx->dev_step_mirror = step;
-  float* grad = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_grad);
-  HaloPlans hp;
-  const HaloPlans* halo = nullptr;
-  if (ctx->halo_mode) {
-    STB_CHECK(ctx->ws == ctx->shared_ws && ctx->shared_ws != nullptr, STB_ERR_STATE,
-              "halo mode needs the library-owned workspace bound (stb_comm_alloc_workspace)");
-    make_plan(ctx, c.rank > 0 ? c.up_h_local : pl.H, pl.W, &hp.up);
-    make_plan(ctx, c.rank + 1 < c.world ? c.dn_h_local : pl.H, pl.W, &hp.dn);
-    halo = &hp;
-  }
-  auto run = [&]() -> int {
-    ctx->halo_seq = 0;
-    STB_TRY(launch_comm_phase(c, 0, s));
-    STB_TRY(launch_halo_pull(c, img, s));
-    STB_TRY(iterate_fwd(ctx, pl, img, s, halo));
-    STB_TRY(launch_stats_allreduce(c, at<float>(ctx, pl.stats_off), pl.stats_floats, s));
-    advance_step_kernel<<<1, 1, 0, s>>>(ctx->d_step);
-    STB_TRY(iterate_bwd(ctx, pl, img, nullptr, nullptr, nullptr, nullptr, 0, grad, loss_out_host8, s, halo));
-    STB_TRY(launch_comm_phase(c, 2, s));
-    STB_TRY(launch_lbfgs_step_banded(state, c, img, ema, ema_decay, halo ? 0 : 1, s));
-    return launch_comm_phase(c, 3, s);
-  };
-  stb_ctx::GraphKey key{};
-  key.H = pl.H; key.W = pl.W; key.ws = ctx->ws; key.img = img; key.m = state; key.ema = ema;
-  key.loss = loss_out_host8; key.decay = ema_decay;
-  return run_graphed(ctx, 5, key, true, s, run);
+  IterArgs a{img, nullptr, nullptr, ema, step};
+  a.ema_decay = ema_decay; a.loss_out_host8 = loss_out_host8; a.state = state; a.state_bytes = state_bytes;
+  return iterate(ctx, kLbfgsBanded, a, true, stream);
 }
 
 // Sync-free loss read-back (SURVEY.md 8f row 2).  host_ring: PINNED host memory of slots x 16 floats (NULL: off).
@@ -1382,14 +1347,15 @@ int stb_graph_status(stb_ctx* ctx, char* note_out, size_t note_bytes) {
   return ctx->graphs_enabled ? (any ? 1 : 2) : 0;  // 2: enabled, nothing captured yet
 }
 
-// Kernel launches issued through graph replays so far (counted from the captured graphs, not assumed): replays,
-// kernels those replays launched, and the kernel nodes of each of the four graph slots (0 where nothing is captured).
+// Kernel launches issued through graph replays so far (counted from the captured graphs, not assumed): replays of every
+// graph, kernels those replays launched, and the kernel nodes of the graphs of stb_iterate, stb_iterate_fwd,
+// stb_iterate_bwd and stb_iterate_banded (0 where nothing is captured; the L-BFGS graphs have no entry).
 int stb_launch_count(stb_ctx* ctx, int64_t* graph_replays, int64_t* kernels_replayed, int* kernels_per_graph4) {
   STB_CHECK(ctx != nullptr, STB_ERR_INVALID, "null ctx");
   if (graph_replays) *graph_replays = ctx->graph_replays;
   if (kernels_replayed) *kernels_replayed = ctx->kernels_replayed;
   if (kernels_per_graph4)
-    for (int i = 0; i < 4; ++i) kernels_per_graph4[i] = ctx->gslot[i].kernel_nodes;   // the ABI's four slots
+    for (int i = GS_ITERATE; i <= GS_ITERATE_BANDED; ++i) kernels_per_graph4[i] = ctx->gslot[i].kernel_nodes;
   return STB_OK;
 }
 

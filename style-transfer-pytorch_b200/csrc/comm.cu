@@ -197,13 +197,7 @@ adam_seam_kernel(CommDev c, float* __restrict__ img, float* __restrict__ exp_avg
     unpack(reinterpret_cast<T*>(img)[idx], pp);
     unpack(reinterpret_cast<T*>(ema)[idx], ee);
 #pragma unroll
-    for (int k = 0; k < V; ++k) {
-      mm[k] = mm[k] + (gg[k] - mm[k]) * ac.one_minus_b1;
-      vv[k] = vv[k] * ac.b2 + ac.one_minus_b2 * gg[k] * gg[k];
-      const float denom = sqrtf(vv[k]) * ac.inv_sqrt_bc2 + ac.eps;
-      pp[k] = fminf(fmaxf(pp[k] - ac.step_size * (mm[k] / denom), 0.f), 1.f);
-      ee[k] = ee[k] * ac.ema_decay + ac.one_minus_decay * pp[k];
-    }
+    for (int k = 0; k < V; ++k) adam_element(ac, gg[k], mm[k], vv[k], pp[k], ee[k]);
     T pn;
     pack(pn, pp);
     pack(reinterpret_cast<T*>(exp_avg)[idx], mm);

@@ -339,12 +339,7 @@ conv0_bwd_kernel(const __grid_constant__ CUtensorMap tm_g0, const bf16* __restri
               if (grad_out) grad_out[idx] = gg;
               if (apply_update) {
                 float mm = cur.m[c], vv = cur.v[c], pp = cur.p[c], ee = cur.e[c];
-                mm = mm + (gg - mm) * ac.one_minus_b1;
-                vv = vv * ac.b2 + ac.one_minus_b2 * gg * gg;
-                const float denom = sqrtf(vv) * ac.inv_sqrt_bc2 + ac.eps;
-                pp = pp - ac.step_size * (mm / denom);
-                pp = fminf(fmaxf(pp, 0.f), 1.f);
-                ee = ee * ac.ema_decay + ac.one_minus_decay * pp;
+                adam_element(ac, gg, mm, vv, pp, ee);
                 exp_avg[idx] = mm; exp_avg_sq[idx] = vv; img[idx] = pp; ema[idx] = ee;
               }
             }

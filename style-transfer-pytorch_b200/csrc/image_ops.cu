@@ -248,12 +248,7 @@ conv0_bwd_adam_kernel(const bf16* __restrict__ g0, const bool interior_done, con
         if (grad_out) grad_out[idx] = g;
         if (apply_update) {
           float m = exp_avg[idx], v = exp_avg_sq[idx], p = img[idx], e = ema[idx];
-          m = m + (g - m) * ac.one_minus_b1;
-          v = v * ac.b2 + ac.one_minus_b2 * g * g;
-          const float denom = sqrtf(v) * ac.inv_sqrt_bc2 + ac.eps;
-          p = p - ac.step_size * (m / denom);
-          p = fminf(fmaxf(p, 0.f), 1.f);
-          e = e * ac.ema_decay + ac.one_minus_decay * p;
+          adam_element(ac, g, m, v, p, e);
           exp_avg[idx] = m; exp_avg_sq[idx] = v; img[idx] = p; ema[idx] = e;
         }
       }

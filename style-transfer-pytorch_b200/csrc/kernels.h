@@ -48,8 +48,29 @@ int pack_weights_bwd(const float* w, bf16* out, int Cout, int Cin, cudaStream_t 
 struct AdamScalars {  // torch/optim/adam.py:413-546 scalars, evaluated on the host in double like torch does
   float one_minus_b1, b2, one_minus_b2, step_size, inv_sqrt_bc2, eps, ema_decay, one_minus_decay;
 };
-// the scalars of Adam step `step` (1-based), as the host-side update paths evaluate them (api.cu)
-AdamScalars make_adam_scalars(int64_t step, float lr, float beta1, float beta2, float adam_eps, float ema_decay);
+// the scalars of Adam step `step` (1-based): on the host for stb_adam_update, on the device by adam_scalars_kernel
+// (each side with its own pow / sqrt)
+__host__ __device__ inline AdamScalars make_adam_scalars(int64_t step, float lr, float beta1, float beta2,
+                                                         float adam_eps, float ema_decay) {
+  AdamScalars as{};
+  const double bc1 = 1.0 - pow((double)beta1, (double)step);
+  const double bc2 = 1.0 - pow((double)beta2, (double)step);
+  as.one_minus_b1 = 1.f - beta1; as.b2 = beta2; as.one_minus_b2 = 1.f - beta2;
+  as.step_size = (float)((double)lr / bc1);
+  as.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2));
+  as.eps = adam_eps; as.ema_decay = ema_decay; as.one_minus_decay = 1.f - ema_decay;
+  return as;
+}
+// Adam + clamp to [0, 1] + EMA of one element: moments m, v, image p, EMA e; g is the gradient.  Every Adam update
+// (conv0's fused epilogues, the band seam, stb_adam_update's rows) runs this one copy, so they all round alike.
+__device__ __forceinline__ void adam_element(const AdamScalars& ac, float g, float& m, float& v, float& p, float& e) {
+  m = m + (g - m) * ac.one_minus_b1;
+  v = v * ac.b2 + ac.one_minus_b2 * g * g;
+  const float denom = sqrtf(v) * ac.inv_sqrt_bc2 + ac.eps;
+  p = p - ac.step_size * (m / denom);
+  p = fminf(fmaxf(p, 0.f), 1.f);
+  e = e * ac.ema_decay + ac.one_minus_decay * p;
+}
 // TV loss partials + gradient (times tv_weight) on the raw image; weights of the tensor-core conv0 in its split
 // K layout (27 hi taps, 27 lo residuals, 10 zeros).
 int launch_tv(const float* img, int H, int W, int row0, int rows, int H_norm, float tv_weight, float* gtv,
