@@ -56,6 +56,18 @@ STB_API int stb_test_w2(const float* mean_t, const float* srm_t, const float* S_
                         float npix, float weight, void* ws, size_t ws_bytes, float* loss_out, float* gs_out,
                         float* gmu_out, float* csqrt_out, void* stream);
 STB_API size_t stb_test_w2_workspace_bytes(void);
+/* the five-layer W2 engine as the iteration drives it, one engine kept per workspace: layer l in slot l (C = 64, 128,
+ * 256, 512, 512), all five problems through the same grouped rounds.  Arrays of five device pointers per layer: target
+ * moments mean_t [C] and srm_t [C][C], statistics S_raw [C][C] and sums [C] (un-normalised sums over npix[l] pixels);
+ * npix and weight are five host floats.  build_targets = 0 reuses the targets of the previous call on the same workspace
+ * (mean_t and srm_t are then not read).  forward_backward runs n_calls >= 1 times; the outputs (device) are those of the
+ * last call: loss_out [5] loss terms, per layer Gs [C][C] fp32 (G + G^T, not divided by npix), gs_bf16 [C][C] (bf16
+ * Gs / npix, what the tap-gradient GEMM reads), gmu [C] (divided by npix), mu [C] and csqrt [C][C] = sqrtm(cov_t). */
+STB_API int stb_test_w2_layers(const float* const* mean_t, const float* const* srm_t, const float* const* S_raw,
+                               const float* const* sums, const float* npix, const float* weight, int build_targets,
+                               int n_calls, void* ws, size_t ws_bytes, float* loss_out, float* const* gs_out,
+                               void* const* gs_bf16_out, float* const* gmu_out, float* const* mu_out,
+                               float* const* csqrt_out, void* stream);
 /* the L-BFGS step of stb_iterate_lbfgs alone (closure replaced by a given gradient, grad NULL: the gradient already held
  * by the state): state of stb_lbfgs_state_bytes(H, W) bytes, x / ema fp32 [3*H*W].  pairs_out / t_out (optional; the
  * call then synchronises the stream): history pairs held and step length of the current direction. */

@@ -79,6 +79,7 @@ def _declare(lib):
 
 def _declare_test(lib):
     vp, i, f, sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    pp = C.POINTER(C.c_void_p)
     lib.stb_test_last_error.restype = C.c_char_p
     lib.stb_test_last_error.argtypes = []
     _set(lib, {
@@ -93,6 +94,7 @@ def _declare_test(lib):
         'stb_test_pool_bwd': [i, vp, vp, vp, i, i, i, vp],
         'stb_test_gram': [vp, C.c_long, i, vp, sz, vp, vp, vp],
         'stb_test_w2': [vp, vp, vp, vp, i, f, f, vp, sz, vp, vp, vp, vp, vp],
+        'stb_test_w2_layers': [pp, pp, pp, pp, C.POINTER(f), C.POINTER(f), i, i, vp, sz, vp, pp, pp, pp, pp, pp, vp],
         'stb_test_lbfgs_step': [vp, sz, i, i, vp, vp, vp, f, C.POINTER(i), C.POINTER(f), vp],
         'stb_test_lbfgs_step_banded': [vp, vp, sz, vp, vp, vp, f, i, C.POINTER(i), C.POINTER(f), vp],
         'stb_test_lbfgs_gradient': [vp, sz, i, i, vp, vp],
@@ -121,7 +123,8 @@ EXPORTS = [
 TEST_EXPORTS = [
     'stb_test_last_error', 'stb_pack_weights', 'stb_test_pixel_gemm', 'stb_test_conv0_fwd', 'stb_test_tv',
     'stb_test_conv0_bwd', 'stb_test_conv0_bwd_adam', 'stb_test_sse', 'stb_test_conv_pool', 'stb_test_pool_bwd', 'stb_test_gram',
-    'stb_test_gram_partials_floats', 'stb_test_w2', 'stb_test_w2_workspace_bytes', 'stb_test_lbfgs_step', 'stb_test_lbfgs_step_banded',
+    'stb_test_gram_partials_floats', 'stb_test_w2', 'stb_test_w2_layers', 'stb_test_w2_workspace_bytes',
+    'stb_test_lbfgs_step', 'stb_test_lbfgs_step_banded',
     'stb_test_lbfgs_gradient', 'stb_test_preload', 'stb_test_comm_info',
 ]
 

@@ -262,4 +262,51 @@ int stb_test_w2(const float* mean_t, const float* srm_t, const float* S_raw, con
   return STB_OK;
 }
 
+// The engine as stb_set_targets / the iteration drive it: five problems in their own slots, S_raw / sums bound in place
+// (as the statistics block is), targets built once and forward_backward run n_calls times on one engine, so that the
+// ping-pong iterates, the scalars and the device-patched Gc alpha carry over from call to call.
+int stb_test_w2_layers(const float* const* mean_t, const float* const* srm_t, const float* const* S_raw,
+                       const float* const* sums, const float* npix, const float* weight, int build_targets,
+                       int n_calls, void* ws, size_t ws_bytes, float* loss_out, float* const* gs_out,
+                       void* const* gs_bf16_out, float* const* gmu_out, float* const* mu_out, float* const* csqrt_out,
+                       void* stream) {
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  static W2Engine eng;  // test-only
+  static void* bound = nullptr;
+  const int ns[5] = {64, 128, 256, 512, 512};
+  STB_CHECK(S_raw && sums && npix && weight && ws && loss_out && gs_out && gs_bf16_out && gmu_out && mu_out &&
+                csqrt_out && n_calls >= 1,
+            STB_ERR_INVALID, "bad argument");
+  STB_CHECK(build_targets || ws == bound, STB_ERR_STATE, "build_targets = 0 needs the workspace of the previous call");
+  if (ws != bound) {
+    STB_TRY(eng.init(ws, ws_bytes, ns));
+    bound = ws;
+  }
+  for (int l = 0; l < 5; ++l) {
+    W2Layer& L = eng.host_layers[l];
+    const size_t nn = (size_t)L.n * L.n;
+    L.weight = weight[l]; L.npix = npix[l];
+    L.S_raw = const_cast<float*>(S_raw[l]);
+    L.sums = const_cast<float*>(sums[l]);
+    if (build_targets) {
+      STB_CHECK(mean_t && srm_t && mean_t[l] && srm_t[l], STB_ERR_INVALID, "build_targets needs mean_t and srm_t");
+      STB_CUDA_CHECK(cudaMemcpyAsync(L.mean_t, mean_t[l], L.n * 4, cudaMemcpyDeviceToDevice, s));
+      STB_CUDA_CHECK(cudaMemcpyAsync(L.srm_t, srm_t[l], nn * 4, cudaMemcpyDeviceToDevice, s));
+    }
+  }
+  STB_TRY(eng.upload_layers(s));
+  if (build_targets) STB_TRY(eng.build_targets(s));
+  for (int c = 0; c < n_calls; ++c) STB_TRY(eng.forward_backward(loss_out, s));
+  for (int l = 0; l < 5; ++l) {
+    const W2Layer& L = eng.host_layers[l];
+    const size_t nn = (size_t)L.n * L.n;
+    STB_CUDA_CHECK(cudaMemcpyAsync(gs_out[l], L.Gs, nn * 4, cudaMemcpyDeviceToDevice, s));
+    STB_CUDA_CHECK(cudaMemcpyAsync(gs_bf16_out[l], L.gs_bf16, nn * 2, cudaMemcpyDeviceToDevice, s));
+    STB_CUDA_CHECK(cudaMemcpyAsync(gmu_out[l], L.gmu_bias, L.n * 4, cudaMemcpyDeviceToDevice, s));
+    STB_CUDA_CHECK(cudaMemcpyAsync(mu_out[l], L.mu, L.n * 4, cudaMemcpyDeviceToDevice, s));
+    STB_TRY(W2Engine::read_matrix(csqrt_out[l], L.P, L.n, s));
+  }
+  return STB_OK;
+}
+
 }  // extern "C"
