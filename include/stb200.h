@@ -38,7 +38,9 @@ extern "C" {
 #define STB_POOL_L2 2      /* Scale(nn.LPPool2d(2, 2), 0.78)  ST:21-22, 41-46 */
 
 #define STB_NUM_CONVS 13      /* VGG-19 features[:30]: convs at 0,2,5,7,10,12,14,16,19,21,23,25,28 */
-#define STB_NUM_STYLE_TAPS 5  /* ReLU outputs 1,6,11,20,29 (ST:317) */
+#define STB_NUM_STYLE_TAPS 5  /* ReLU outputs 1,6,11,20,29 (ST:317): the default style layers */
+#define STB_NUM_TAPS 6        /* ReLU outputs 1,6,11,20,22,29: the taps of the reference model (ST:324) */
+#define STB_MAX_LOSS_TERMS 14 /* total + 6 content + 6 style + TV */
 
 typedef struct stb_ctx stb_ctx;
 
@@ -59,6 +61,17 @@ STB_API void stb_ctx_destroy(stb_ctx* ctx);
 STB_API int stb_workspace_bytes(stb_ctx* ctx, int H, int W, size_t* bytes);
 STB_API int stb_bind_workspace(stb_ctx* ctx, void* ptr, size_t bytes, void* stream);
 
+/* ------------------------------------------------------------------ layer table (StyleTransfer.content_layers,
+ * style_layers; ST:316-317, 365-455).  content_layers: 1 to 6 taps, style_layers: 0 to 6 taps, each from the six
+ * ReLU taps {1, 6, 11, 20, 22, 29} of the reference model, no tap twice in one list (a tap may be in both lists).
+ * The order of each list is the order of the per-layer arrays of the calls below and of the loss terms.
+ * STB_ERR_INVALID for anything else, before any state changes.  The call resets the graphs, invalidates the targets
+ * and re-lays the W2 engine out over the style taps; stb_workspace_bytes then reflects the table (activations are
+ * kept through the deepest configured conv only; a content target at tap 1 is H x W x 64 bf16, 537 MB at 2048^2).
+ * An iteration runs the forward through the conv of the deepest configured tap and starts the backward there.
+ * A context that never calls it has the default table: content [22], style [1, 6, 11, 20, 29]. */
+STB_API int stb_set_layers(stb_ctx* ctx, int n_content, const int* content_layers, int n_style, const int* style_layers);
+
 /* ------------------------------------------------------------------ target extraction (no-grad VGG forward)
  * stb_style_stats      = self.model(style, layers=style_layers) + StyleLossW2.get_target   (ST:440-443, 163-168)
  *                        mean_out[l]: [C_l] fp32, srm_out[l]: [C_l,C_l] fp32, l over taps 1,6,11,20,29
@@ -68,6 +81,11 @@ STB_API int stb_bind_workspace(stb_ctx* ctx, void* ptr, size_t bytes, void* stre
 STB_API int stb_style_stats(stb_ctx* ctx, const float* img, int H, int W, float* const* mean_out,
                             float* const* srm_out, void* stream);
 STB_API int stb_content_features(stb_ctx* ctx, const float* img, int H, int W, void* target_out_bf16, void* stream);
+/* Under the context's layer table: stb_style_stats fills one (mean, srm) pair per style tap, in table order (nothing
+ * without style taps); stb_content_features_ex one bf16 NHWC target [h_l][w_l][C_l] per content tap.
+ * stb_content_features / stb_set_targets are the default table's calls (STB_ERR_STATE under any other table). */
+STB_API int stb_content_features_ex(stb_ctx* ctx, const float* img, int H, int W, void* const* targets_out,
+                                    void* stream);
 
 /* ------------------------------------------------------------------ per-scale loss state (ST:426-455)
  * mean_t/srm_t: the style-weight-blended target moments (ST:443-450); the library forms cov = srm - mean mean^T
@@ -75,6 +93,16 @@ STB_API int stb_content_features(stb_ctx* ctx, const float* img, int H, int W, v
 STB_API int stb_set_targets(stb_ctx* ctx, int H, int W, const void* content_target_bf16, float content_weight,
                             const float* const* mean_t, const float* const* srm_t, const float* style_w,
                             float tv_weight, float eps, void* stream);
+/* Per-layer arrays in table order: content_targets / content_w (content_weight / len(content_layers), ST:366) per
+ * content tap; mean_t / srm_t / style_w per style tap. */
+STB_API int stb_set_targets_ex(stb_ctx* ctx, int H, int W, const void* const* content_targets, const float* content_w,
+                               const float* const* mean_t, const float* const* srm_t, const float* style_w,
+                               float tv_weight, float eps, void* stream);
+/* The loss-term vector of the last iteration, [total, content terms..., style terms..., tv] in table order: 2 +
+ * n_content + n_style <= STB_MAX_LOSS_TERMS floats ({loss, content, style1..5, tv} for the default table).
+ * *n_terms receives the count; min(count, capacity) floats are copied, stream-ordered, into host memory `out`.
+ * loss_out_host8 of the iteration calls receives the first eight words of this vector. */
+STB_API int stb_loss_terms(stb_ctx* ctx, float* out, int capacity, int* n_terms, void* stream);
 
 /* ------------------------------------------------------------------ THE HOT PATH: one iteration of ST:480-486
  * forward + losses + backward + Adam(lr, betas, eps; bias correction with `step` = 1-based count carried across
@@ -126,8 +154,9 @@ STB_API int stb_adam_update(float* img, const float* grad, float* exp_avg, float
                             float ema_decay, void* stream);
 
 /* ------------------------------------------------------------------ sync-free loss read-back (ST:487-493)
- * host_ring: PINNED host memory, slots x 16 floats (NULL switches it off).  Each updating iteration stores its eight
- * terms into slot (step % slots) and then the step as the slot's int32 stamp (word 8), from the loss kernel itself,
+ * host_ring: PINNED host memory, slots x 16 floats (NULL switches it off).  Each updating iteration stores its loss-term
+ * vector (stb_loss_terms) into slot (step % slots), term k at word k for k < 8 and at word k + 1 above, and then the
+ * step as the slot's int32 stamp (word 8), from the loss kernel itself,
  * BEFORE the backward pass starts: the host polls the stamp -- the per-iteration callback needs no stream sync and
  * overlaps the rest of the iteration. */
 STB_API int stb_set_loss_ring(stb_ctx* ctx, float* host_ring, int slots);

@@ -13,6 +13,7 @@ LIB_PATH = Path(os.environ.get('STB_LIB', PKG_DIR / 'libstb200.so'))   # STB_LIB
 TEST_LIB_PATH = PKG_DIR / 'libstb200_test.so'
 
 STB_ERR_INVALID = -1
+MAX_LOSS_TERMS = 14   # STB_MAX_LOSS_TERMS
 POOLING = {'max': 0, 'average': 1, 'l2': 2}
 
 _lib = None
@@ -42,6 +43,10 @@ def _declare(lib):
         'stb_style_stats': [vp, vp, i, i, pp, pp, vp],
         'stb_content_features': [vp, vp, i, i, vp, vp],
         'stb_set_targets': [vp, i, i, vp, f, pp, pp, C.POINTER(f), f, f, vp],
+        'stb_set_layers': [vp, i, C.POINTER(i), i, C.POINTER(i)],
+        'stb_content_features_ex': [vp, vp, i, i, pp, vp],
+        'stb_set_targets_ex': [vp, i, i, pp, C.POINTER(f), pp, pp, C.POINTER(f), f, f, vp],
+        'stb_loss_terms': [vp, vp, i, C.POINTER(i), vp],
         'stb_iterate': [vp, vp, vp, vp, vp, i64, f, f, f, f, f, vp, vp],
         'stb_iterate_ex': [vp, vp, vp, vp, vp, i64, f, f, f, f, f, i, vp, vp, vp],
         'stb_lbfgs_state_bytes': [i, i, C.POINTER(sz)],
@@ -112,6 +117,7 @@ def _declare_test(lib):
 EXPORTS = [
     'stb_last_error', 'stb_ctx_create', 'stb_ctx_destroy', 'stb_workspace_bytes', 'stb_bind_workspace',
     'stb_style_stats', 'stb_content_features', 'stb_set_targets', 'stb_iterate', 'stb_iterate_ex',
+    'stb_set_layers', 'stb_content_features_ex', 'stb_set_targets_ex', 'stb_loss_terms',
     'stb_lbfgs_state_bytes', 'stb_lbfgs_reset', 'stb_iterate_lbfgs',
     'stb_set_band', 'stb_stats_block', 'stb_iterate_fwd', 'stb_iterate_bwd', 'stb_adam_update',
     'stb_set_loss_ring', 'stb_resize', 'stb_comm_create', 'stb_comm_connect_ipc', 'stb_comm_connect_local', 'stb_comm_disconnect', 'stb_comm_alloc_workspace',

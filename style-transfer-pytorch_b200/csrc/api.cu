@@ -20,11 +20,63 @@ constexpr int NCONV = STB_NUM_CONVS;
 const int kCin[NCONV] = {3, 64, 64, 128, 128, 256, 256, 256, 256, 512, 512, 512, 512};
 const int kCout[NCONV] = {64, 64, 128, 128, 256, 256, 256, 256, 512, 512, 512, 512, 512};
 const bool kPoolAfter[NCONV] = {false, true, false, true, false, false, false, true, false, false, false, true, false};
-const int kStyleConv[5] = {0, 2, 4, 8, 12};  // convs whose ReLU output is style tap 1, 6, 11, 20, 29 (ST:317)
-constexpr int kContentConv = 9;              // relu4_2 = layer 22 (ST:316)
-const int kStyleC[5] = {64, 128, 256, 512, 512};
+// The six ReLU taps of the reference model, VGGFeatures(style_layers + content_layers) with the default lists (ST:324),
+// and the convs whose ReLU output they are.  A layer table selects content and style taps among them.
+constexpr int kNumTaps = STB_NUM_TAPS;
+const int kTapLayer[kNumTaps] = {1, 6, 11, 20, 22, 29};
+const int kTapConv[kNumTaps] = {0, 2, 4, 8, 9, 12};
+constexpr int kStatsTailMax = 8;    // the stats tail of the largest table: six content SSEs + TV, padded to 4 floats
+constexpr int kSsePartials = 1024;  // launch_sse writes at most this many partials
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// content and style taps in the caller's list order (stb_set_layers); the default is the reference's (ST:316-317)
+struct LayerTable {
+  int n_content = 1, content_conv[kNumTaps] = {9};
+  int n_style = 5, style_conv[kNumTaps] = {0, 2, 4, 8, 12};
+  int style_c(int l) const;
+  int last_conv() const {   // the deepest conv any loss term reads: the forward stops there, the backward starts there
+    int last = 0;
+    for (int k = 0; k < n_content; ++k) last = std::max(last, content_conv[k]);
+    for (int l = 0; l < n_style; ++l) last = std::max(last, style_conv[l]);
+    return last;
+  }
+  int last_style_conv() const {
+    int last = 0;
+    for (int l = 0; l < n_style; ++l) last = std::max(last, style_conv[l]);
+    return last;
+  }
+  int last_content_conv() const {
+    int last = 0;
+    for (int k = 0; k < n_content; ++k) last = std::max(last, content_conv[k]);
+    return last;
+  }
+  int style_at(int conv) const {   // style index of the tap at `conv`, or -1
+    for (int l = 0; l < n_style; ++l) if (style_conv[l] == conv) return l;
+    return -1;
+  }
+  int content_at(int conv) const {
+    for (int k = 0; k < n_content; ++k) if (content_conv[k] == conv) return k;
+    return -1;
+  }
+  bool is_default() const {
+    const LayerTable d;
+    return n_content == d.n_content && n_style == d.n_style &&
+           std::memcmp(content_conv, d.content_conv, sizeof(int) * n_content) == 0 &&
+           std::memcmp(style_conv, d.style_conv, sizeof(int) * n_style) == 0;
+  }
+  // {content SSE per content tap, TV sum} ride at the tail of the stats block, padded to four floats
+  size_t stats_tail() const { return align_up((size_t)n_content + 1, 4); }
+};
+
+int LayerTable::style_c(int l) const { return kCout[style_conv[l]]; }
+
+// the stats block of the largest configuration (all six taps in both roles): the size of a mailbox's stats slots
+size_t stats_floats_max() {
+  size_t sf = kStatsTailMax;
+  for (int t = 0; t < kNumTaps; ++t) sf += (size_t)kCout[kTapConv[t]] * kCout[kTapConv[t]] + kCout[kTapConv[t]];
+  return sf;
+}
 
 struct Plan {
   int H = 0, W = 0;
@@ -32,8 +84,9 @@ struct Plan {
   size_t act_off[NCONV];       // post-ReLU output of conv i (bf16 NHWC)
   size_t pool_off[4];          // pooled copies
   size_t g_off[2];             // gradient ping-pong
-  size_t gtv_off, tvp_off, ssep_off, gramp_off, stats_off, loss_off, ctarget_off;
-  size_t stats_layer_off[5];   // in floats, inside the stats block: S_raw then sums per layer
+  size_t gtv_off, tvp_off, ssep_off, gramp_off, stats_off, loss_off;
+  size_t ctarget_off[kNumTaps];        // content target of each content tap (bf16 NHWC)
+  size_t stats_layer_off[kNumTaps];    // in floats, inside the stats block: S_raw then sums per style tap
   size_t stats_scalars = 0, stats_floats = 0, gramp_floats = 0;
   size_t total = 0;
   int n_tv_partials = 0, n_sse_partials = 0;
@@ -92,8 +145,8 @@ struct stb_ctx {
   // per-scale loss state
   bool targets_set = false;
   int tH = 0, tW = 0;
-  float content_weight = 0.f, tv_weight = 0.f;
-  float style_w[5] = {};
+  LayerTable layers;
+  float content_w[kNumTaps] = {}, tv_weight = 0.f;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   // spatial tiling (multi-GPU): this context works on a horizontal band of a taller image.  The local image is the
   // band plus halo aprons; only the "own" rows contribute to the statistics / losses / tap gradients.
@@ -152,7 +205,10 @@ struct stb_ctx {
 
 namespace {
 
+// workspace layout for an H x W image under the context's layer table: activations up to its deepest conv only
 void make_plan(const stb_ctx* ctx, int H, int W, Plan* pl) {
+  const LayerTable& lt = ctx->layers;
+  const int last = lt.last_conv();
   pl->H = H; pl->W = W;
   int h = H, w = W;
   size_t off = align_up(ctx->w2_bytes, 1024);
@@ -161,11 +217,11 @@ void make_plan(const stb_ctx* ctx, int H, int W, Plan* pl) {
   size_t gmax = 0;
   for (int i = 0; i < NCONV; ++i) {
     pl->h[i] = h; pl->w[i] = w;
-    pl->act_off[i] = take((size_t)h * w * kCout[i] * 2);
-    gmax = std::max(gmax, (size_t)h * w * kCout[i] * 2);
+    pl->act_off[i] = i <= last ? take((size_t)h * w * kCout[i] * 2) : 0;
+    if (i <= last) gmax = std::max(gmax, (size_t)h * w * kCout[i] * 2);
     if (kPoolAfter[i]) {
       h /= 2; w /= 2;
-      pl->pool_off[np++] = take((size_t)std::max(h, 1) * std::max(w, 1) * kCout[i] * 2);
+      pl->pool_off[np++] = i < last ? take((size_t)std::max(h, 1) * std::max(w, 1) * kCout[i] * 2) : 0;
     }
   }
   pl->g_off[0] = take(gmax);
@@ -173,21 +229,28 @@ void make_plan(const stb_ctx* ctx, int H, int W, Plan* pl) {
   pl->gtv_off = take((size_t)3 * H * W * 4);
   pl->n_tv_partials = ((W + 255) / 256) * H;
   pl->tvp_off = take((size_t)pl->n_tv_partials * 4);
-  pl->ssep_off = take(1024 * 4);
+  pl->ssep_off = take((size_t)kSsePartials * lt.n_content * 4);   // the SSE partials of content tap k at k * 1024
   // split-K partials of the Gram kernels: the bound over every pixel count, because a banded context launches them
   // on its own rows only and the split count is not monotonic in the pixel count (~40 MB)
   size_t gp = 0;
-  for (int l = 0; l < 5; ++l) gp = std::max(gp, gram_max_partials_floats(kStyleC[l]));
+  for (int l = 0; l < lt.n_style; ++l) gp = std::max(gp, gram_max_partials_floats(lt.style_c(l)));
   pl->gramp_floats = gp;
   pl->gramp_off = take(gp * 4);
   size_t sf = 0;
-  for (int l = 0; l < 5; ++l) { pl->stats_layer_off[l] = sf; sf += (size_t)kStyleC[l] * kStyleC[l] + kStyleC[l]; }
-  pl->stats_scalars = sf;  // {content SSE, TV sum, 0, 0} ride at the tail so that one all-reduce covers everything
-  sf += 4;
+  for (int l = 0; l < lt.n_style; ++l) {
+    const int C = lt.style_c(l);
+    pl->stats_layer_off[l] = sf;
+    sf += (size_t)C * C + C;
+  }
+  pl->stats_scalars = sf;  // {content SSE per content tap, TV sum} ride at the tail: one all-reduce covers everything
+  sf += lt.stats_tail();
   pl->stats_floats = sf;
   pl->stats_off = take(sf * 4);
   pl->loss_off = take(64 * 4);
-  pl->ctarget_off = take((size_t)pl->h[kContentConv] * pl->w[kContentConv] * 512 * 2);
+  for (int k = 0; k < lt.n_content; ++k) {
+    const int ci = lt.content_conv[k];
+    pl->ctarget_off[k] = take((size_t)pl->h[ci] * pl->w[ci] * kCout[ci] * 2);
+  }
   pl->total = off;
 }
 
@@ -308,9 +371,10 @@ int forward(stb_ctx* ctx, const Plan& pl, const float* img, int last_conv, bool 
 int style_grams(stb_ctx* ctx, const Plan& pl, cudaStream_t s) {
   float* stats = at<float>(ctx, pl.stats_off);
   ctx->prof.begin(PC_GRAM, s);
-  for (int l = 0; l < 5; ++l) {
-    const int ci = kStyleConv[l];
-    const int C = kStyleC[l];
+  const LayerTable& lt = ctx->layers;
+  for (int l = 0; l < lt.n_style; ++l) {
+    const int ci = lt.style_conv[l];
+    const int C = lt.style_c(l);
     float* S = stats + pl.stats_layer_off[l];
     const BandRows br = band_rows(ctx, pl, ci);
     STB_TRY(launch_gram(at<bf16>(ctx, pl.act_off[ci]) + (size_t)br.own0 * pl.w[ci] * C, (long)br.rows * pl.w[ci], C,
@@ -320,21 +384,41 @@ int style_grams(stb_ctx* ctx, const Plan& pl, cudaStream_t s) {
   return STB_OK;
 }
 
-// deterministic single-block reduction of the content-SSE and TV partials into the stats tail
-__global__ void reduce2_kernel(const float* __restrict__ a, int na, const float* __restrict__ b, int nb,
-                               float* __restrict__ out) {
-  __shared__ float s_red[2][32];
-  float sa = 0.f, sb = 0.f;
-  for (int i = threadIdx.x; i < na; i += blockDim.x) sa += a[i];
-  for (int i = threadIdx.x; i < nb; i += blockDim.x) sb += b[i];
-  sa = warp_sum(sa);
-  sb = warp_sum(sb);
-  if ((threadIdx.x & 31) == 0) { s_red[0][threadIdx.x >> 5] = sa; s_red[1][threadIdx.x >> 5] = sb; }
+// deterministic single-block reduction of the partials of every content SSE and of TV into the stats tail:
+// out[j] = sum of array j (each summed in the same fixed order), zeros up to `tail` words
+struct PartialArrays {
+  const float* p[kNumTaps + 1];
+  int n[kNumTaps + 1];
+  int count, tail;
+};
+__global__ void reduce_partials_kernel(PartialArrays a, float* __restrict__ out) {
+  __shared__ float s_red[kNumTaps + 1][32];
+  for (int j = 0; j < a.count; ++j) {
+    float v = 0.f;
+    for (int i = threadIdx.x; i < a.n[j]; i += blockDim.x) v += a.p[j][i];
+    v = warp_sum(v);
+    if ((threadIdx.x & 31) == 0) s_red[j][threadIdx.x >> 5] = v;
+  }
   __syncthreads();
   if (threadIdx.x == 0) {
-    float ta = 0.f, tb = 0.f;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { ta += s_red[0][i]; tb += s_red[1][i]; }
-    out[0] = ta; out[1] = tb; out[2] = 0.f; out[3] = 0.f;
+    for (int j = 0; j < a.count; ++j) {
+      float t = 0.f;
+      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += s_red[j][i];
+      out[j] = t;
+    }
+    for (int j = a.count; j < a.tail; ++j) out[j] = 0.f;
+  }
+}
+
+// the first loss term of the content-only tap that seeds the backward (no style role there, so no GEMM): d loss /
+// d pre-activation = (y > 0) * cscale * (y - t) on rows [row_lo, row_hi) of [rows][w][C], zero elsewhere
+__global__ void content_seed_kernel(const bf16* __restrict__ y, const bf16* __restrict__ t, bf16* __restrict__ g,
+                                    long n, long row_elems, int row_lo, int row_hi, float cscale) {
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const int row = (int)(i / row_elems);
+    const float yv = __bfloat162float(y[i]);
+    const float v = (row >= row_lo && row < row_hi) ? cscale * (yv - __bfloat162float(t[i])) : 0.f;
+    g[i] = __float2bfloat16(yv > 0.f ? v : 0.f);
   }
 }
 
@@ -370,32 +454,48 @@ __global__ void scale_copy_kernel(const float* __restrict__ in, float* __restric
     out[i] = in[i] * scale;
 }
 
-// loss = cw * sse / numel + sum_l style_l + tvw * tv   (python sum, left to right, ST:208/455)
-// `ring` (optional): pinned HOST memory, slots x 16 floats.  The kernel stores the eight terms into slot
-// (step % slots) and then, after a system-scope fence, the step itself as the slot's stamp (word 8): the host polls the
-// stamp instead of synchronising the stream, so the callback of iteration i overlaps the backward pass of iteration i.
-__global__ void finalize_loss_kernel(const float* __restrict__ scalars, float content_scale,
+// terms = [total, content_k * cw_k / numel_k ..., style_l ..., tvw * tv]; total = their python sum, left to right
+// (SumLoss, ST:208/455).  `ring` (optional): pinned HOST memory, slots x 16 floats.  The kernel stores term k into word
+// k (k < 8) or k + 1 (k >= 8) of slot (step % slots) and then, after a system-scope fence, the step itself as the
+// slot's stamp (word 8): the host polls the stamp instead of synchronising the stream, so the callback of iteration i
+// overlaps the backward pass of iteration i.
+struct ContentScales { float s[kNumTaps]; int n_content, n_style; };
+__global__ void finalize_loss_kernel(const float* __restrict__ scalars, ContentScales cs,
                                      const float* __restrict__ style_terms, float tv_weight,
                                      float* __restrict__ out, float* ring, int ring_slots,
                                      const long long* __restrict__ d_step) {
   if (threadIdx.x == 0) {
-    const float content = scalars[0] * content_scale;
-    const float tv = scalars[1] * tv_weight;
-    float loss = content;
-    for (int l = 0; l < 5; ++l) loss += style_terms[l];
+    const int nc = cs.n_content, ns = cs.n_style;
+    float loss = 0.f;
+    for (int k = 0; k < nc; ++k) {
+      const float content = scalars[k] * cs.s[k];
+      loss = k == 0 ? content : loss + content;
+      out[1 + k] = content;
+    }
+    for (int l = 0; l < ns; ++l) {
+      loss += style_terms[l];
+      out[1 + nc + l] = style_terms[l];
+    }
+    const float tv = scalars[nc] * tv_weight;
     loss += tv;
     out[0] = loss;
-    out[1] = content;
-    for (int l = 0; l < 5; ++l) out[2 + l] = style_terms[l];
-    out[7] = tv;
+    out[1 + nc + ns] = tv;
     if (ring != nullptr && d_step != nullptr) {
       const long long step = *d_step;
       volatile float* slot = ring + (size_t)(step % ring_slots) * 16;
-      for (int i = 0; i < 8; ++i) slot[i] = out[i];
+      for (int i = 0; i < 2 + nc + ns; ++i) slot[i < 8 ? i : i + 1] = out[i];
       __threadfence_system();
       reinterpret_cast<volatile int*>(slot)[8] = (int)step;
     }
   }
+}
+
+// the W2 engine over the style taps of the layer table, in the fixed W2 block at the head of the workspace
+int init_w2(stb_ctx* ctx) {
+  const LayerTable& lt = ctx->layers;
+  int cs[kNumTaps];
+  for (int l = 0; l < lt.n_style; ++l) cs[l] = lt.style_c(l);
+  return ctx->w2.init(ctx->ws, ctx->w2_bytes, lt.n_style, cs);
 }
 
 void comm_release(stb_ctx* ctx) {
@@ -518,26 +618,63 @@ int stb_bind_workspace(stb_ctx* ctx, void* ptr, size_t bytes, void* stream) {
   ctx->ws_bytes = bytes;
   ctx->reset_graphs();
   ctx->targets_set = false;
-  STB_TRY(ctx->w2.init(ctx->ws, ctx->w2_bytes, kStyleC));
+  STB_TRY(init_w2(ctx));
   ctx->w2_ready = true;
+  return STB_OK;
+}
+
+int stb_set_layers(stb_ctx* ctx, int n_content, const int* content_layers, int n_style, const int* style_layers) {
+  STB_CHECK(ctx != nullptr, STB_ERR_INVALID, "null ctx");
+  STB_CHECK(n_content >= 1 && n_content <= kNumTaps && content_layers != nullptr, STB_ERR_INVALID,
+            "content_layers must list 1 to %d taps, got %d", kNumTaps, n_content);
+  STB_CHECK(n_style >= 0 && n_style <= kNumTaps && (n_style == 0 || style_layers != nullptr), STB_ERR_INVALID,
+            "style_layers must list 0 to %d taps, got %d", kNumTaps, n_style);
+  LayerTable lt;
+  auto to_conv = [](const int* layers, int n, int* conv_out, const char* what) -> int {
+    for (int k = 0; k < n; ++k) {
+      int t = 0;
+      while (t < kNumTaps && kTapLayer[t] != layers[k]) ++t;
+      STB_CHECK(t < kNumTaps, STB_ERR_INVALID, "%s: layer %d is not one of the taps 1, 6, 11, 20, 22, 29", what,
+                layers[k]);
+      for (int j = 0; j < k; ++j)
+        STB_CHECK(layers[j] != layers[k], STB_ERR_INVALID, "%s: layer %d is listed twice", what, layers[k]);
+      conv_out[k] = kTapConv[t];
+    }
+    return STB_OK;
+  };
+  STB_TRY(to_conv(content_layers, n_content, lt.content_conv, "content_layers"));
+  STB_TRY(to_conv(style_layers, n_style, lt.style_conv, "style_layers"));
+  lt.n_content = n_content;
+  lt.n_style = n_style;
+  STB_ENTER(ctx);
+  ctx->layers = lt;
+  ctx->reset_graphs();
+  ctx->targets_set = false;
+  if (ctx->ws != nullptr) {
+    ctx->w2_ready = false;
+    STB_TRY(init_w2(ctx));
+    ctx->w2_ready = true;
+  }
   return STB_OK;
 }
 
 int stb_style_stats(stb_ctx* ctx, const float* img, int H, int W, float* const* mean_out, float* const* srm_out,
                     void* stream) {
-  STB_CHECK(ctx && img && mean_out && srm_out, STB_ERR_INVALID, "null argument");
+  STB_CHECK(ctx && img && (ctx->layers.n_style == 0 || (mean_out && srm_out)), STB_ERR_INVALID, "null argument");
   STB_ENTER(ctx);
-  STB_TRY(check_size(H, W, NCONV - 1));
+  const LayerTable& lt = ctx->layers;
+  if (lt.n_style == 0) return STB_OK;
+  STB_TRY(check_size(H, W, lt.last_style_conv()));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   Plan pl;
   make_plan(ctx, H, W, &pl);
   STB_TRY(ensure_ws(ctx, pl));
-  STB_TRY(forward(ctx, pl, img, NCONV - 1, false, s));
+  STB_TRY(forward(ctx, pl, img, lt.last_style_conv(), false, s));
   STB_TRY(style_grams(ctx, pl, s));
   const float* stats = at<float>(ctx, pl.stats_off);
-  for (int l = 0; l < 5; ++l) {
-    const int C = kStyleC[l];
-    const int ci = kStyleConv[l];
+  for (int l = 0; l < lt.n_style; ++l) {
+    const int C = lt.style_c(l);
+    const int ci = lt.style_conv[l];
     // banded contexts return RAW sums over their own rows (the host all-reduces and normalises by the global count)
     const float inv = ctx->band_on ? 1.f : 1.f / ((float)pl.h[ci] * (float)pl.w[ci]);
     const float* S = stats + pl.stats_layer_off[l];
@@ -548,40 +685,58 @@ int stb_style_stats(stb_ctx* ctx, const float* img, int H, int W, float* const* 
   return STB_OK;
 }
 
-int stb_content_features(stb_ctx* ctx, const float* img, int H, int W, void* target_out_bf16, void* stream) {
-  STB_CHECK(ctx && img && target_out_bf16, STB_ERR_INVALID, "null argument");
+int stb_content_features_ex(stb_ctx* ctx, const float* img, int H, int W, void* const* targets_out, void* stream) {
+  STB_CHECK(ctx && img && targets_out, STB_ERR_INVALID, "null argument");
   STB_ENTER(ctx);
-  STB_TRY(check_size(H, W, kContentConv));
+  const LayerTable& lt = ctx->layers;
+  for (int k = 0; k < lt.n_content; ++k) STB_CHECK(targets_out[k] != nullptr, STB_ERR_INVALID, "null target %d", k);
+  STB_TRY(check_size(H, W, lt.last_content_conv()));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   Plan pl;
   make_plan(ctx, H, W, &pl);
   STB_TRY(ensure_ws(ctx, pl));
-  STB_TRY(forward(ctx, pl, img, kContentConv, false, s));
-  const size_t bytes = (size_t)pl.h[kContentConv] * pl.w[kContentConv] * 512 * 2;
-  STB_CUDA_CHECK(cudaMemcpyAsync(target_out_bf16, at<bf16>(ctx, pl.act_off[kContentConv]), bytes,
-                                 cudaMemcpyDeviceToDevice, s));
+  STB_TRY(forward(ctx, pl, img, lt.last_content_conv(), false, s));
+  for (int k = 0; k < lt.n_content; ++k) {
+    const int ci = lt.content_conv[k];
+    const size_t bytes = (size_t)pl.h[ci] * pl.w[ci] * kCout[ci] * 2;
+    STB_CUDA_CHECK(cudaMemcpyAsync(targets_out[k], at<bf16>(ctx, pl.act_off[ci]), bytes, cudaMemcpyDeviceToDevice, s));
+  }
   return STB_OK;
 }
 
-int stb_set_targets(stb_ctx* ctx, int H, int W, const void* content_target_bf16, float content_weight,
-                    const float* const* mean_t, const float* const* srm_t, const float* style_w, float tv_weight,
-                    float eps, void* stream) {
-  STB_CHECK(ctx && content_target_bf16 && mean_t && srm_t && style_w, STB_ERR_INVALID, "null argument");
+int stb_content_features(stb_ctx* ctx, const float* img, int H, int W, void* target_out_bf16, void* stream) {
+  STB_CHECK(ctx && target_out_bf16, STB_ERR_INVALID, "null argument");
+  STB_CHECK(ctx->layers.is_default(), STB_ERR_STATE, "stb_content_features needs the default layers (use _ex)");
+  return stb_content_features_ex(ctx, img, H, W, &target_out_bf16, stream);
+}
+
+int stb_set_targets_ex(stb_ctx* ctx, int H, int W, const void* const* content_targets, const float* content_w,
+                       const float* const* mean_t, const float* const* srm_t, const float* style_w, float tv_weight,
+                       float eps, void* stream) {
+  const LayerTable& lt = ctx ? ctx->layers : LayerTable{};
+  STB_CHECK(ctx && content_targets && content_w && (lt.n_style == 0 || (mean_t && srm_t && style_w)), STB_ERR_INVALID,
+            "null argument");
+  for (int k = 0; k < lt.n_content; ++k) STB_CHECK(content_targets[k] != nullptr, STB_ERR_INVALID, "null target %d", k);
   STB_ENTER(ctx);
-  STB_TRY(check_size(H, W, NCONV - 1));
+  STB_TRY(check_size(H, W, NCONV - 1));   // the closure's model holds all six taps (ST:324, 473)
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   Plan pl;
   make_plan(ctx, H, W, &pl);
   STB_TRY(ensure_ws(ctx, pl));
   STB_CHECK(ctx->w2_ready, STB_ERR_STATE, "workspace not bound");
   ctx->reset_graphs();  // weights are baked into the graphs
-  const size_t cbytes = (size_t)pl.h[kContentConv] * pl.w[kContentConv] * 512 * 2;
-  STB_CUDA_CHECK(cudaMemcpyAsync(at<bf16>(ctx, pl.ctarget_off), content_target_bf16, cbytes, cudaMemcpyDeviceToDevice, s));
+  for (int k = 0; k < lt.n_content; ++k) {
+    const int ci = lt.content_conv[k];
+    const size_t cbytes = (size_t)pl.h[ci] * pl.w[ci] * kCout[ci] * 2;
+    STB_CUDA_CHECK(cudaMemcpyAsync(at<bf16>(ctx, pl.ctarget_off[k]), content_targets[k], cbytes,
+                                   cudaMemcpyDeviceToDevice, s));
+    ctx->content_w[k] = content_w[k];
+  }
   float* stats = at<float>(ctx, pl.stats_off);
-  for (int l = 0; l < 5; ++l) {
+  for (int l = 0; l < lt.n_style; ++l) {
     W2Layer& L = ctx->w2.host_layers[l];
-    const int C = kStyleC[l];
-    const int ci = kStyleConv[l];
+    const int C = lt.style_c(l);
+    const int ci = lt.style_conv[l];
     L.eps = eps;
     L.weight = style_w[l];
     L.npix = (float)band_rows(ctx, pl, ci).h_global * (float)pl.w[ci];
@@ -589,16 +744,37 @@ int stb_set_targets(stb_ctx* ctx, int H, int W, const void* content_target_bf16,
     L.sums = L.S_raw + (size_t)C * C;
     STB_CUDA_CHECK(cudaMemcpyAsync(L.mean_t, mean_t[l], (size_t)C * 4, cudaMemcpyDeviceToDevice, s));
     STB_CUDA_CHECK(cudaMemcpyAsync(L.srm_t, srm_t[l], (size_t)C * C * 4, cudaMemcpyDeviceToDevice, s));
-    ctx->style_w[l] = style_w[l];
   }
   STB_TRY(ctx->w2.upload_layers(s));
   STB_TRY(ctx->w2.build_targets(s));
   if (ctx->band_on)  // TV gradient of the halo rows belongs to the neighbouring band: keep it zero here
     STB_CUDA_CHECK(cudaMemsetAsync(at<float>(ctx, pl.gtv_off), 0, (size_t)3 * H * W * 4, s));
-  ctx->content_weight = content_weight;
   ctx->tv_weight = tv_weight;
   ctx->tH = H; ctx->tW = W;
   ctx->targets_set = true;
+  return STB_OK;
+}
+
+int stb_set_targets(stb_ctx* ctx, int H, int W, const void* content_target_bf16, float content_weight,
+                    const float* const* mean_t, const float* const* srm_t, const float* style_w, float tv_weight,
+                    float eps, void* stream) {
+  STB_CHECK(ctx && content_target_bf16, STB_ERR_INVALID, "null argument");
+  STB_CHECK(ctx->layers.is_default(), STB_ERR_STATE, "stb_set_targets needs the default layers (use _ex)");
+  return stb_set_targets_ex(ctx, H, W, &content_target_bf16, &content_weight, mean_t, srm_t, style_w, tv_weight, eps,
+                            stream);
+}
+
+int stb_loss_terms(stb_ctx* ctx, float* out, int capacity, int* n_terms, void* stream) {
+  STB_CHECK(ctx && n_terms && (out || capacity == 0) && capacity >= 0, STB_ERR_INVALID, "bad argument");
+  STB_ENTER(ctx);
+  STB_CHECK(ctx->targets_set, STB_ERR_STATE, "stb_set_targets must precede stb_loss_terms");
+  const int n = 2 + ctx->layers.n_content + ctx->layers.n_style;
+  *n_terms = n;
+  if (capacity == 0) return STB_OK;
+  Plan pl;
+  make_plan(ctx, ctx->tH, ctx->tW, &pl);
+  STB_CUDA_CHECK(cudaMemcpyAsync(out, at<float>(ctx, pl.loss_off), sizeof(float) * std::min(n, capacity),
+                                 cudaMemcpyDeviceToHost, static_cast<cudaStream_t>(stream)));
   return STB_OK;
 }
 
@@ -608,17 +784,24 @@ namespace {
 
 // phase 1: forward + this context's (band-local) statistics into the stats block
 int iterate_fwd(stb_ctx* ctx, const Plan& pl, const float* img, cudaStream_t s, const HaloPlans* halo) {
-  STB_TRY(forward(ctx, pl, img, NCONV - 1, true, s, halo));
+  const LayerTable& lt = ctx->layers;
+  STB_TRY(forward(ctx, pl, img, lt.last_conv(), true, s, halo));
   STB_TRY(style_grams(ctx, pl, s));
-  const BandRows b22 = band_rows(ctx, pl, kContentConv);
-  const size_t off22 = (size_t)b22.own0 * pl.w[kContentConv] * 512;
-  const long n22_local = (long)b22.rows * pl.w[kContentConv] * 512;
-  int n_sse = 0;
+  PartialArrays parts{};
   ctx->prof.begin(PC_SSE, s);
-  STB_TRY(launch_sse(at<bf16>(ctx, pl.act_off[kContentConv]) + off22, at<bf16>(ctx, pl.ctarget_off) + off22, n22_local,
-                     at<float>(ctx, pl.ssep_off), &n_sse, s));
-  reduce2_kernel<<<1, 1024, 0, s>>>(at<float>(ctx, pl.ssep_off), n_sse, at<float>(ctx, pl.tvp_off), ctx->n_tv_partials,
-                                    at<float>(ctx, pl.stats_off) + pl.stats_scalars);
+  for (int k = 0; k < lt.n_content; ++k) {
+    const int ci = lt.content_conv[k], C = kCout[ci];
+    const BandRows b = band_rows(ctx, pl, ci);
+    const size_t off = (size_t)b.own0 * pl.w[ci] * C;
+    parts.p[k] = at<float>(ctx, pl.ssep_off) + (size_t)k * kSsePartials;
+    STB_TRY(launch_sse(at<bf16>(ctx, pl.act_off[ci]) + off, at<bf16>(ctx, pl.ctarget_off[k]) + off,
+                       (long)b.rows * pl.w[ci] * C, const_cast<float*>(parts.p[k]), &parts.n[k], s));
+  }
+  parts.p[lt.n_content] = at<float>(ctx, pl.tvp_off);
+  parts.n[lt.n_content] = ctx->n_tv_partials;
+  parts.count = lt.n_content + 1;
+  parts.tail = (int)lt.stats_tail();
+  reduce_partials_kernel<<<1, 1024, 0, s>>>(parts, at<float>(ctx, pl.stats_off) + pl.stats_scalars);
   ctx->prof.end(s);
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
@@ -632,41 +815,66 @@ struct FusedAdam { float *exp_avg, *exp_avg_sq, *ema; const AdamScalars* d_adam;
 int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, const FusedAdam* update, bool publish_loss, float* grad_out,
                 float* loss_out_host8, cudaStream_t s, const HaloPlans* halo) {
   const int H = pl.H, W = pl.W;
-  const long n22 = (long)band_rows(ctx, pl, kContentConv).h_global * pl.w[kContentConv] * 512;  // global numel
+  const LayerTable& lt = ctx->layers;
+  // 2 * content weight / numel of content tap k (global numel under tiling): the scale of its dgrad injection
+  auto content_numel = [&](int k) {
+    const int ci = lt.content_conv[k];
+    return (long)band_rows(ctx, pl, ci).h_global * pl.w[ci] * kCout[ci];
+  };
   float* loss_dev = at<float>(ctx, pl.loss_off);
   ctx->prof.begin(PC_W2, s);
   STB_TRY(ctx->w2.forward_backward(loss_dev + 16, s));
   ctx->prof.end(s);
   // every loss term is known here (content SSE and TV from the forward, the style terms from the W2 forward): assemble
   // and publish the loss BEFORE the backward pass, so a host callback can consume it while the device works on
+  ContentScales cs{};
+  cs.n_content = lt.n_content; cs.n_style = lt.n_style;
+  for (int k = 0; k < lt.n_content; ++k) cs.s[k] = ctx->content_w[k] / (float)content_numel(k);
   ctx->prof.begin(PC_FINALIZE, s);
-  finalize_loss_kernel<<<1, 32, 0, s>>>(at<float>(ctx, pl.stats_off) + pl.stats_scalars,
-                                        ctx->content_weight / (float)n22, loss_dev + 16, ctx->tv_weight, loss_dev,
-                                        publish_loss ? ctx->ring_dev : nullptr, ctx->ring_slots, ctx->d_step);
+  finalize_loss_kernel<<<1, 32, 0, s>>>(at<float>(ctx, pl.stats_off) + pl.stats_scalars, cs, loss_dev + 16,
+                                        ctx->tv_weight, loss_dev, publish_loss ? ctx->ring_dev : nullptr,
+                                        ctx->ring_slots, ctx->d_step);
   ctx->prof.end(s);
   if (loss_out_host8)
     STB_CUDA_CHECK(cudaMemcpyAsync(loss_out_host8, loss_dev, 8 * sizeof(float), cudaMemcpyDeviceToHost, s));
 
   bf16* g[2] = {at<bf16>(ctx, pl.g_off[0]), at<bf16>(ctx, pl.g_off[1])};
   int cur = 0;
-  {  // tap 29: d loss / d conv12 pre-activation = mask * (F Gs / N + gmu / N), own rows only
-    const W2Layer& L = ctx->w2.host_layers[4];
-    const BandRows br = band_rows(ctx, pl, 12);
-    PixelGemmArgs a;
-    a.H = pl.h[12]; a.W = pl.w[12]; a.Cin = 0; a.Cout = 512; a.C2 = 512; a.mode = 1;
-    a.A2 = at<bf16>(ctx, pl.act_off[12]) + (size_t)br.own0 * pl.w[12] * 512;
-    a.a2_row0 = br.own0; a.a2_rows = br.rows; a.row_lo = br.own0; a.row_hi = br.own0 + br.rows;
-    a.B2 = L.gs_bf16; a.bias = L.gmu_bias;
-    a.mask_src = at<bf16>(ctx, pl.act_off[12]); a.out = g[cur];
-    if (halo) { a.y_origin = br.own0; a.y_rows = br.rows; }
+  const int last = lt.last_conv();
+  {  // the deepest tap: d loss / d pre-activation of its conv, own rows only.  With a style role it is
+     // mask * (F Gs / N + gmu / N) [+ the content injection], a pixel GEMM on the tap alone; content only: the seed kernel
+    const BandRows br = band_rows(ctx, pl, last);
+    const int C = kCout[last], ls = lt.style_at(last), kc = lt.content_at(last);
     ctx->prof.begin(PC_CONV_BWD, s);
-    STB_TRY(launch_pixel_gemm(a, s));
+    if (ls >= 0) {
+      const W2Layer& L = ctx->w2.host_layers[ls];
+      PixelGemmArgs a;
+      a.H = pl.h[last]; a.W = pl.w[last]; a.Cin = 0; a.Cout = C; a.C2 = C; a.mode = 1;
+      a.A2 = at<bf16>(ctx, pl.act_off[last]) + (size_t)br.own0 * pl.w[last] * C;
+      a.a2_row0 = br.own0; a.a2_rows = br.rows; a.row_lo = br.own0; a.row_hi = br.own0 + br.rows;
+      a.B2 = L.gs_bf16; a.bias = L.gmu_bias;
+      a.mask_src = at<bf16>(ctx, pl.act_off[last]); a.out = g[cur];
+      if (kc >= 0) {
+        a.ctarget = at<bf16>(ctx, pl.ctarget_off[kc]);
+        a.cscale = 2.f * ctx->content_w[kc] / (float)content_numel(kc);
+      }
+      if (halo) { a.y_origin = br.own0; a.y_rows = br.rows; }
+      STB_TRY(launch_pixel_gemm(a, s));
+    } else {
+      const long row_elems = (long)pl.w[last] * C, n = (long)pl.h[last] * row_elems;
+      long blocks = (n + 255) / 256;
+      if (blocks > 16l * num_sms()) blocks = 16l * num_sms();
+      content_seed_kernel<<<(unsigned)blocks, 256, 0, s>>>(
+          at<bf16>(ctx, pl.act_off[last]), at<bf16>(ctx, pl.ctarget_off[kc]), g[cur], n, row_elems, br.own0,
+          br.own0 + br.rows, 2.f * ctx->content_w[kc] / (float)content_numel(kc));
+      STB_CUDA_CHECK(cudaGetLastError());
+    }
     ctx->prof.end(s);
     if (halo)
-      STB_TRY(halo_exchange(ctx, level_of(12), pl.w[12], 512, pl.g_off[cur], halo->up.g_off[cur], halo->dn.g_off[cur],
-                            false, s));
+      STB_TRY(halo_exchange(ctx, level_of(last), pl.w[last], C, pl.g_off[cur], halo->up.g_off[cur],
+                            halo->dn.g_off[cur], false, s));
   }
-  for (int i = NCONV - 1; i >= 1; --i) {
+  for (int i = last; i >= 1; --i) {
     // g[cur] = gradient w.r.t. conv i pre-activation, [h_i][w_i][Cout_i]; produce gradient for conv i-1
     PixelGemmArgs a;
     a.H = pl.h[i]; a.W = pl.w[i]; a.Cin = kCout[i]; a.Cout = kCin[i];
@@ -703,17 +911,17 @@ int iterate_bwd(stb_ctx* ctx, const Plan& pl, float* img, const FusedAdam* updat
       a.mask_src = at<bf16>(ctx, pl.act_off[i - 1]);
       const BandRows br = band_rows(ctx, pl, i - 1);
       a.row_lo = br.own0; a.row_hi = br.own0 + br.rows;
-      for (int l = 0; l < 5; ++l)
-        if (kStyleConv[l] == i - 1) {
-          const W2Layer& L = ctx->w2.host_layers[l];
-          a.C2 = kStyleC[l];
-          a.A2 = at<bf16>(ctx, pl.act_off[i - 1]) + (size_t)br.own0 * pl.w[i - 1] * kStyleC[l];
-          a.a2_row0 = br.own0; a.a2_rows = br.rows;
-          a.B2 = L.gs_bf16; a.bias = L.gmu_bias;
-        }
-      if (i - 1 == kContentConv) {
-        a.ctarget = at<bf16>(ctx, pl.ctarget_off);
-        a.cscale = 2.f * ctx->content_weight / (float)n22;
+      const int ls = lt.style_at(i - 1), kc = lt.content_at(i - 1);
+      if (ls >= 0) {
+        const W2Layer& L = ctx->w2.host_layers[ls];
+        a.C2 = lt.style_c(ls);
+        a.A2 = at<bf16>(ctx, pl.act_off[i - 1]) + (size_t)br.own0 * pl.w[i - 1] * a.C2;
+        a.a2_row0 = br.own0; a.a2_rows = br.rows;
+        a.B2 = L.gs_bf16; a.bias = L.gmu_bias;
+      }
+      if (kc >= 0) {
+        a.ctarget = at<bf16>(ctx, pl.ctarget_off[kc]);
+        a.cscale = 2.f * ctx->content_w[kc] / (float)content_numel(kc);
       }
       ctx->prof.begin(PC_CONV_BWD, s);
       STB_TRY(launch_pixel_gemm(a, s));
@@ -1086,10 +1294,9 @@ int stb_comm_create(stb_ctx* ctx, int rank, int world, int max_h_local, int max_
   STB_CUDA_CHECK(cudaDeviceSynchronize());
   comm_release(ctx);
   ctx->reset_graphs();
-  Plan pl;
-  make_plan(ctx, 16, 16, &pl);  // stats block size does not depend on the image size
   size_t off[5];
-  ctx->comm_bytes = comm_mailbox_bytes(pl.stats_floats, max_h_local, max_W, off);
+  // stats slots for the largest layer table, so that stb_set_layers never has to re-create a mailbox
+  ctx->comm_bytes = comm_mailbox_bytes(stats_floats_max(), max_h_local, max_W, off);
   STB_CUDA_CHECK(cudaMalloc(&ctx->comm_mailbox, ctx->comm_bytes));
   STB_CUDA_CHECK(cudaMemset(ctx->comm_mailbox, 0, ctx->comm_bytes));
   STB_CUDA_CHECK(cudaDeviceSynchronize());
@@ -1113,7 +1320,8 @@ int stb_comm_create(stb_ctx* ctx, int rank, int world, int max_h_local, int max_
   STB_TRY(comm_preload()); STB_TRY(preload_conv_kernels()); STB_TRY(preload_gram_kernels());
   STB_TRY(preload_w2_kernels()); STB_TRY(preload_conv0_kernels()); STB_TRY(preload_image_kernels());
   cudaFuncAttributes fa;
-  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(reduce2_kernel)));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(reduce_partials_kernel)));
+  STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(content_seed_kernel)));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(adam_scalars_kernel)));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(finalize_loss_kernel)));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(advance_step_kernel)));
@@ -1372,7 +1580,8 @@ int stb_debug_w2_trace(stb_ctx* ctx, unsigned long long* host_out, size_t words,
 
 // test hook: copy an internal activation (post-ReLU output of conv `conv_index`, bf16 NHWC) of the last forward
 int stb_debug_activation(stb_ctx* ctx, int H, int W, int conv_index, void* out_bf16, size_t out_bytes, void* stream) {
-  STB_CHECK(ctx && out_bf16 && conv_index >= 0 && conv_index < NCONV, STB_ERR_INVALID, "bad argument");
+  STB_CHECK(ctx && out_bf16 && conv_index >= 0 && conv_index <= ctx->layers.last_conv(), STB_ERR_INVALID,
+            "bad argument (conv %d: the forward runs through conv %d)", conv_index, ctx ? ctx->layers.last_conv() : 0);
   Plan pl;
   make_plan(ctx, H, W, &pl);
   STB_TRY(ensure_ws(ctx, pl));

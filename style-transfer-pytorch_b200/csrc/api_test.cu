@@ -225,7 +225,7 @@ int stb_test_w2(const float* mean_t, const float* srm_t, const float* S_raw, con
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   static W2Engine eng;  // test-only
   const int ns[5] = {64, 128, 256, 512, 512};
-  STB_TRY(eng.init(ws, ws_bytes, ns));
+  STB_TRY(eng.init(ws, ws_bytes, 5, ns));
   int slot = -1;
   for (int l = 0; l < 5; ++l)
     if (ns[l] == C) { slot = l; break; }
@@ -279,7 +279,7 @@ int stb_test_w2_layers(const float* const* mean_t, const float* const* srm_t, co
             STB_ERR_INVALID, "bad argument");
   STB_CHECK(build_targets || ws == bound, STB_ERR_STATE, "build_targets = 0 needs the workspace of the previous call");
   if (ws != bound) {
-    STB_TRY(eng.init(ws, ws_bytes, ns));
+    STB_TRY(eng.init(ws, ws_bytes, 5, ns));
     bound = ws;
   }
   for (int l = 0; l < 5; ++l) {

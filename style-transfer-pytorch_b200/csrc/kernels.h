@@ -140,7 +140,8 @@ struct TcProb {  // D = alpha * A * B + gamma * I, all n x n row-major; a matrix
   int in_half;  // operands are fp16 plane pairs (hi, lo * 2^11) instead of TF32 pairs: kind::f16 MMAs, half the bytes
   int out_half; // D is written as an fp16 plane pair
 };
-constexpr int W2_MAX_PROBS = 10, W2_MAX_TILES = 152, W2_TRACE_WORDS = 8 * 128;
+// a round holds up to two problems per layer; six layers of 64, 128, 256, 512, 512, 512 channels give 214 tiles
+constexpr int W2_MAX_LAYERS = 6, W2_MAX_PROBS = 2 * W2_MAX_LAYERS, W2_MAX_TILES = 216, W2_TRACE_WORDS = 8 * 128;
 struct W2Round {  // one grouped GEMM step of all layers; lives in device memory, walked by w2_chain_kernel
   int n_tiles, n_probs;
   TcProb probs[W2_MAX_PROBS];
@@ -165,7 +166,8 @@ struct W2Layer {
   float* red;       // reduction partials {sum of squares, trace} x 128
 };
 struct W2Engine {
-  W2Layer host_layers[5];
+  int n_layers = 0;
+  W2Layer host_layers[W2_MAX_LAYERS];
   W2Layer* d_layers = nullptr;
   CUtensorMap* d_maps = nullptr;
   W2Round* d_rounds = nullptr;        // device copy of `rounds` (the chain kernel walks it)
@@ -176,11 +178,12 @@ struct W2Engine {
       r_bwd_end = 0, gc_round = 0;
   static size_t layer_floats(int n);
   static size_t workspace_bytes();
-  int init(void* ws, size_t bytes, const int n_per_layer[5]);
+  // n_layers (0..W2_MAX_LAYERS) problems of n_per_layer[l] channels each, in {64, 128, 256, 512}
+  int init(void* ws, size_t bytes, int n_layers, const int* n_per_layer);
   int upload_layers(cudaStream_t s);           // after editing host_layers (weights, npix, S_raw/sums pointers)
   int run_rounds(int r0, int r1, cudaStream_t s);
   int build_targets(cudaStream_t s);            // mean_t/srm_t -> cov_t, P = sqrtm_ns(cov_t)   (ST:152-160)
-  int forward_backward(float* loss_terms, cudaStream_t s);  // S_raw/sums -> loss_terms[5], gs_bf16, gmu_bias
+  int forward_backward(float* loss_terms, cudaStream_t s);  // S_raw/sums -> loss_terms[n_layers], gs_bf16, gmu_bias
   static int read_matrix(float* dst, const float* pair, int n, cudaStream_t s);  // dst = hi + lo (test hook)
 };
 

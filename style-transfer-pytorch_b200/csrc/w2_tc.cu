@@ -29,6 +29,7 @@
 // Tensor maps are encoded once per workspace binding.
 #include <cuda_fp16.h>
 
+#include <algorithm>
 #include <cstdlib>
 #include <map>
 #include <set>
@@ -571,9 +572,10 @@ size_t W2Engine::layer_floats(int n) {
 }
 
 size_t W2Engine::workspace_bytes() {
+  // the largest configuration: all six style taps of the reference model, 1, 6, 11, 20, 22 and 29
   size_t fl = 0;
-  const int ns[5] = {64, 128, 256, 512, 512};
-  for (int l = 0; l < 5; ++l) fl += layer_floats(ns[l]) + (size_t)ns[l] * ns[l] / 2 + 64;  // + bf16 Gs
+  const int ns[W2_MAX_LAYERS] = {64, 128, 256, 512, 512, 512};
+  for (int l = 0; l < W2_MAX_LAYERS; ++l) fl += layer_floats(ns[l]) + (size_t)ns[l] * ns[l] / 2 + 64;  // + bf16 Gs
   // + device copies of the layer table, tensor maps, problems and tiles
   return fl * 4 + (size_t(1) << 20);
 }
@@ -635,15 +637,20 @@ struct Builder {
     ++R.n_probs;
   }
 };
-constexpr int MAX_MAPS = 5 * 32 * 4;
+constexpr int MAX_MAPS = W2_MAX_LAYERS * 32 * 4;
 }  // namespace
 
-int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
+int W2Engine::init(void* ws, size_t bytes, int nl, const int* n_per_layer) {
   STB_CHECK(bytes >= workspace_bytes(), STB_ERR_WORKSPACE, "W2 workspace too small");
+  STB_CHECK(nl >= 0 && nl <= W2_MAX_LAYERS, STB_ERR_INVALID, "W2: %d layers (at most %d)", nl, W2_MAX_LAYERS);
+  for (int l = 0; l < nl; ++l)
+    STB_CHECK(n_per_layer[l] == 64 || n_per_layer[l] == 128 || n_per_layer[l] == 256 || n_per_layer[l] == 512,
+              STB_ERR_INVALID, "W2: %d channels (64, 128, 256 or 512)", n_per_layer[l]);
+  n_layers = nl;
   uint8_t* base = static_cast<uint8_t*>(ws);
   size_t off = 0;
   auto take = [&](size_t nbytes) { void* p = base + off; off += (nbytes + 255) & ~size_t(255); return p; };
-  for (int l = 0; l < 5; ++l) {
+  for (int l = 0; l < nl; ++l) {
     W2Layer& L = host_layers[l];
     const int n = n_per_layer[l];
     const size_t nn = (size_t)n * n * 4, pp = 4 * nn;  // single plane / (hi, lo, hi^T, lo^T)
@@ -663,7 +670,7 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
     L.gs_bf16 = (bf16*)take((size_t)n * n * 2);
     L.weight = 0.f; L.npix = 1.f;
   }
-  d_layers = (W2Layer*)take(sizeof(W2Layer) * 5);
+  d_layers = (W2Layer*)take(sizeof(W2Layer) * W2_MAX_LAYERS);
   d_maps = (CUtensorMap*)take(sizeof(CUtensorMap) * MAX_MAPS);
   d_grid_counter = (unsigned*)take(256);
   d_trace = (unsigned long long*)take(W2_TRACE_WORDS * 8);
@@ -673,7 +680,7 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
   b.d_maps = d_maps;
   b.rounds = &rounds;
   rounds.clear();
-  for (int l = 0; l < 5; ++l) {  // the normalised iterates of both iterations live as fp16 plane pairs
+  for (int l = 0; l < nl; ++l) {  // the normalised iterates of both iterations live as fp16 plane pairs
     W2Layer& L = host_layers[l];
     for (float* m : {L.Y[0], L.Y[1], L.Z[0], L.Z[1], L.T, L.A[0], L.A[1], L.Q[0], L.Q[1], L.E}) b.half_mats.insert(m);
   }
@@ -683,10 +690,10 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
     for (int it = 0; it < 12; ++it) {
       const int s = it & 1, d = s ^ 1;
       begin_round();
-      for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.T, L.Z[s], L.Y[s], -0.5f, 1.5f); }
+      for (int l = nl - 1; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.T, L.Z[s], L.Y[s], -0.5f, 1.5f); }
       end_round();
       begin_round();
-      for (int l = 4; l >= 0; --l) {  // largest matrices first: the tiles beyond one per SM are short ones
+      for (int l = nl - 1; l >= 0; --l) {  // largest matrices first: the tiles beyond one per SM are short ones
         W2Layer& L = host_layers[l];
         b.add(L.n, L.Y[d], L.Y[s], L.T, 1.f, 0.f, it == 11 ? L.red : nullptr);
         if (it < 11) b.add(L.n, L.Z[d], L.T, L.Z[s], 1.f);  // Z is dead after the last Y
@@ -701,10 +708,10 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
   // (b) iterate forward: X = P cov; M = X P; NS
   r_fwd_begin = (int)rounds.size();
   begin_round();
-  for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.X, L.P, L.cov, 1.f, 0.f, nullptr, 0); }
+  for (int l = nl - 1; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.X, L.P, L.cov, 1.f, 0.f, nullptr, 0); }
   end_round();
   begin_round();
-  for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.M, L.X, L.P, 1.f, 0.f, L.red, 1); }  // M^T planes: ns_init reads them coalesced
+  for (int l = nl - 1; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.M, L.X, L.P, 1.f, 0.f, L.red, 1); }  // M^T planes: ns_init reads them coalesced
   end_round();
   r_fwd_ns_begin = (int)rounds.size();
   ns_rounds();
@@ -717,10 +724,10 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
   for (int it = 0; it < 12; ++it) {
     const int s = it & 1, d = s ^ 1;
     begin_round();
-    for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.E, L.A[s], L.A[s], -1.f, 3.f); }
+    for (int l = nl - 1; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.E, L.A[s], L.A[s], -1.f, 3.f); }
     end_round();
     begin_round();
-    for (int l = 4; l >= 0; --l) {
+    for (int l = nl - 1; l >= 0; --l) {
       W2Layer& L = host_layers[l];
       b.add(L.n, it == 11 ? L.Qf : L.Q[d], L.Q[s], L.E, 0.5f);   // the final q leaves the iteration as a TF32 pair
       if (it < 11) b.add(L.n, L.A[d], L.A[s], L.E, 0.5f);
@@ -730,30 +737,34 @@ int W2Engine::init(void* ws, size_t bytes, const int n_per_layer[5]) {
   // after 12 its q (times the layer's power-of-two q scale) is in Qf.  U = P^T q ; Gc = alpha U P^T + (w/C) I with
   // alpha = 0.5 / qscale patched on the device by w2_fwd_finish_kernel, gamma per layer in upload_layers
   begin_round();
-  for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.U, L.P, L.Qf, 1.f, 0.f, nullptr, 0, 1, 0); }
+  for (int l = nl - 1; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.U, L.P, L.Qf, 1.f, 0.f, nullptr, 0, 1, 0); }
   end_round();
   begin_round();
   gc_round = (int)rounds.size() - 1;
-  for (int l = 4; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.Gc, L.U, L.P, 0.5f, 0.f, nullptr, 0, 0, 1); }
+  for (int l = nl - 1; l >= 0; --l) { W2Layer& L = host_layers[l]; b.add(L.n, L.Gc, L.U, L.P, 0.5f, 0.f, nullptr, 0, 0, 1); }
   end_round();
   r_bwd_end = (int)rounds.size();
   STB_CHECK(b.rc == 0, STB_ERR_CUDA, "W2 round construction failed (%d): %s", b.rc, last_error_string().c_str());
   STB_CHECK((int)b.maps.size() <= MAX_MAPS, STB_ERR_WORKSPACE, "W2 tensor map table overflow (%zu)", b.maps.size());
 
-  d_rounds = (W2Round*)take(sizeof(W2Round) * rounds.size());
+  d_rounds = (W2Round*)take(sizeof(W2Round) * std::max<size_t>(rounds.size(), 1));
   STB_CHECK(off <= bytes, STB_ERR_WORKSPACE, "W2 workspace overflow (%zu > %zu)", off, bytes);
   STB_CUDA_CHECK(cudaMemcpy(d_rounds, rounds.data(), sizeof(W2Round) * rounds.size(), cudaMemcpyHostToDevice));
-  for (int l = 0; l < 5; ++l) host_layers[l].gc_alpha = &d_rounds[gc_round].probs[4 - l].alpha;
+  // the rounds list the layers deepest first: layer l is problem nl - 1 - l of the Gc round
+  for (int l = 0; l < nl; ++l) host_layers[l].gc_alpha = &d_rounds[gc_round].probs[nl - 1 - l].alpha;
+  if (nl == 0) return STB_OK;
   STB_CUDA_CHECK(cudaMemcpy(d_maps, b.maps.data(), sizeof(CUtensorMap) * b.maps.size(), cudaMemcpyHostToDevice));
-  STB_CUDA_CHECK(cudaMemcpy(d_layers, host_layers, sizeof(W2Layer) * 5, cudaMemcpyHostToDevice));
+  STB_CUDA_CHECK(cudaMemcpy(d_layers, host_layers, sizeof(W2Layer) * nl, cudaMemcpyHostToDevice));
   return STB_OK;
 }
 
 int W2Engine::upload_layers(cudaStream_t s) {
   // layer weights enter the Gc round through gamma = w / C (rounds travel as kernel parameters)
-  for (int l = 0; l < 5; ++l) rounds[gc_round].probs[4 - l].gamma = host_layers[l].weight / host_layers[l].n;
+  if (n_layers == 0) return STB_OK;
+  for (int l = 0; l < n_layers; ++l)
+    rounds[gc_round].probs[n_layers - 1 - l].gamma = host_layers[l].weight / host_layers[l].n;
   STB_CUDA_CHECK(cudaMemcpyAsync(d_rounds + gc_round, &rounds[gc_round], sizeof(W2Round), cudaMemcpyHostToDevice, s));
-  STB_CUDA_CHECK(cudaMemcpyAsync(d_layers, host_layers, sizeof(W2Layer) * 5, cudaMemcpyHostToDevice, s));
+  STB_CUDA_CHECK(cudaMemcpyAsync(d_layers, host_layers, sizeof(W2Layer) * n_layers, cudaMemcpyHostToDevice, s));
   return STB_OK;
 }
 
@@ -794,7 +805,8 @@ int W2Engine::run_rounds(int r0, int r1, cudaStream_t s) {
 
 int W2Engine::build_targets(cudaStream_t s) {
   // srm_t / mean_t already hold the blended target moments (ST:443-450)
-  const dim3 grid(5, NB);
+  if (n_layers == 0) return STB_OK;
+  const dim3 grid(n_layers, NB);
   w2_cov_kernel<<<grid, 256, 0, s>>>(d_layers, 1);
   w2_ns_init_kernel<<<grid, 256, 0, s>>>(d_layers, 1);
   STB_TRY(run_rounds(r_target_begin, r_target_end, s));
@@ -804,7 +816,8 @@ int W2Engine::build_targets(cudaStream_t s) {
 }
 
 int W2Engine::forward_backward(float* loss_terms, cudaStream_t s) {
-  const dim3 grid(5, NB);
+  if (n_layers == 0) return STB_OK;
+  const dim3 grid(n_layers, NB);
   w2_cov_kernel<<<grid, 256, 0, s>>>(d_layers, 0);
   STB_TRY(run_rounds(r_fwd_begin, r_fwd_ns_begin, s));
   w2_ns_init_kernel<<<grid, 256, 0, s>>>(d_layers, 0);

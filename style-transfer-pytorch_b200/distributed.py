@@ -240,10 +240,16 @@ def local_slice(full: torch.Tensor, band: Band):
     return full[:, :, band.loc_begin:band.loc_end].contiguous()
 
 
-def tap_pixel_counts(h: int, w: int):
-    """Pixels of the five style taps (relu1_1 ... relu5_1) of an h x w image: four floor-mode 2x2 pools."""
+# pyramid level (floor-mode 2x2 pools before it) of each ReLU tap of the reference model
+TAP_LEVEL = {1: 0, 6: 1, 11: 2, 20: 3, 22: 3, 29: 4}
+
+
+def tap_pixel_counts(h: int, w: int, taps=(1, 6, 11, 20, 29)):
+    """Pixels of the given ReLU taps (default: the five default style taps) of an h x w image."""
     out = []
-    for _ in range(5):
-        out.append(h * w)
-        h, w = h // 2, w // 2
+    for t in taps:
+        hl, wl = h, w
+        for _ in range(TAP_LEVEL[t]):
+            hl, wl = hl // 2, wl // 2
+        out.append(hl * wl)
     return out

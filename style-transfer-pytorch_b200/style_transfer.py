@@ -30,6 +30,23 @@ CONV_CHANNELS = [(3, 64), (64, 64), (64, 128), (128, 128), (128, 256), (256, 256
                  (256, 512), (512, 512), (512, 512), (512, 512), (512, 512)]
 VGG19_CONV_INDICES = [0, 2, 5, 7, 10, 12, 14, 16, 19, 21, 23, 25, 28]
 STYLE_CHANNELS = [64, 128, 256, 512, 512]
+# the ReLU taps of the reference model, VGGFeatures(style_layers + content_layers) with its default lists (ST:324), and
+# their channel counts: content_layers and style_layers may name any of them
+TAP_CHANNELS = {1: 64, 6: 128, 11: 256, 20: 512, 22: 512, 29: 512}
+TAP_LEVEL = D.TAP_LEVEL
+
+
+def check_layers(content_layers, style_layers):
+    """Validate StyleTransfer.content_layers / style_layers: KeyError(layer) for a tap the reference model does not
+    have (its LayerApply raises the same, ST:234), ValueError for a tap listed twice in one list (the reference would
+    count a repeated style layer's target statistics twice, ST:442-450).  An empty content list raises
+    ZeroDivisionError earlier, where the content weight is divided by its length (ST:366)."""
+    for name, layers in (('content_layers', content_layers), ('style_layers', style_layers)):
+        for layer in layers:
+            if layer not in TAP_CHANNELS:
+                raise KeyError(layer)
+        if len(set(layers)) != len(layers):
+            raise ValueError(f'{name} lists a layer twice: {list(layers)}')
 
 
 @dataclass
@@ -197,21 +214,51 @@ class NativeVGG:
             raise ValueError(f'expected a [1,3,H,W] image, got {tuple(image.shape)}')
         return image.detach().to(self.device, torch.float32).contiguous()
 
+    def set_layers(self, content_layers, style_layers):
+        """The context's layer table (stb_set_layers): content and style taps, in list order."""
+        content_layers, style_layers = [int(t) for t in content_layers], [int(t) for t in style_layers]
+        check_layers(content_layers, style_layers)
+        ca = (ctypes.c_int * max(len(content_layers), 1))(*content_layers)
+        sa = (ctypes.c_int * max(len(style_layers), 1))(*style_layers)
+        _lib.check(self.lib.stb_set_layers(self.ctx, len(content_layers), ca, len(style_layers), sa))
+        self.content_layers, self.style_layers = content_layers, style_layers
+
+    content_layers = [22]               # the table of a context that never called set_layers
+    style_layers = [1, 6, 11, 20, 29]
+
+    @property
+    def n_terms(self):
+        """Length of the loss-term vector [total, content terms, style terms, tv] under the layer table."""
+        return 2 + len(self.content_layers) + len(self.style_layers)
+
     def style_stats(self, image):
+        """(means, second raw moments) of one image, one pair per style tap of the layer table."""
         image = self._check_image(image)
         _, _, h, w = image.shape
-        means = [torch.empty(c, device=self.device) for c in STYLE_CHANNELS]
-        srms = [torch.empty(c, c, device=self.device) for c in STYLE_CHANNELS]
+        chans = [TAP_CHANNELS[t] for t in self.style_layers]
+        means = [torch.empty(c, device=self.device) for c in chans]
+        srms = [torch.empty(c, c, device=self.device) for c in chans]
         mp, _k1 = _lib.ptr_array(means)
         sp, _k2 = _lib.ptr_array(srms)
         _lib.check(self.lib.stb_style_stats(self.ctx, _lib.ptr(image), h, w, mp, sp, _lib.cur_stream()))
         return means, srms
 
     def content_features(self, image):
+        """The content target of the default layer table (tap 22, bf16 NHWC [H/8][W/8][512])."""
         image = self._check_image(image)
         _, _, h, w = image.shape
         out = torch.empty(h // 8, w // 8, 512, dtype=torch.bfloat16, device=self.device)
         _lib.check(self.lib.stb_content_features(self.ctx, _lib.ptr(image), h, w, _lib.ptr(out), _lib.cur_stream()))
+        return out
+
+    def content_features_list(self, image):
+        """One bf16 NHWC target per content tap of the layer table."""
+        image = self._check_image(image)
+        _, _, h, w = image.shape
+        out = [torch.empty(h >> TAP_LEVEL[t], w >> TAP_LEVEL[t], TAP_CHANNELS[t], dtype=torch.bfloat16,
+                           device=self.device) for t in self.content_layers]
+        op, _k = _lib.ptr_array(out)
+        _lib.check(self.lib.stb_content_features_ex(self.ctx, _lib.ptr(image), h, w, op, _lib.cur_stream()))
         return out
 
     # ------------------------------------------------------------------ spatial tiling (multi-GPU) plumbing
@@ -294,11 +341,30 @@ class NativeVGG:
         return a.value, b.value, list(per)
 
     def set_targets(self, h, w, content_target, content_weight, means, srms, layer_weights, tv_weight, eps=1e-4):
+        """Targets of the default layer table: one content target, five style taps."""
         mp, _k1 = _lib.ptr_array(means)
         sp, _k2 = _lib.ptr_array(srms)
         lw = (ctypes.c_float * 5)(*layer_weights)
         _lib.check(self.lib.stb_set_targets(self.ctx, h, w, _lib.ptr(content_target), content_weight, mp, sp, lw,
                                             tv_weight, eps, _lib.cur_stream()))
+
+    def set_targets_list(self, h, w, content_targets, content_weights, means, srms, layer_weights, tv_weight,
+                         eps=1e-4):
+        """Per-layer lists in layer-table order: content targets and weights, style moments and layer weights."""
+        cp, _k0 = _lib.ptr_array(content_targets)
+        cw = (ctypes.c_float * len(content_weights))(*content_weights)
+        mp, _k1 = _lib.ptr_array(means)
+        sp, _k2 = _lib.ptr_array(srms)
+        lw = (ctypes.c_float * max(len(layer_weights), 1))(*layer_weights)
+        _lib.check(self.lib.stb_set_targets_ex(self.ctx, h, w, cp, cw, mp, sp, lw, tv_weight, eps, _lib.cur_stream()))
+
+    def loss_terms(self):
+        """[total, content terms, style terms, tv] of the last iteration (synchronises the current stream)."""
+        out = torch.zeros(_lib.MAX_LOSS_TERMS, dtype=torch.float32)
+        n = ctypes.c_int()
+        _lib.check(self.lib.stb_loss_terms(self.ctx, _lib.ptr(out), out.numel(), ctypes.byref(n), _lib.cur_stream()))
+        torch.cuda.current_stream().synchronize()
+        return out[:n.value].clone()
 
 
 class _Stopped(Exception):
@@ -687,15 +753,18 @@ class StyleTransfer:
         m.set_band(True, sh, band.own0, band.own_rows)
         means, srms = m.style_stats(D.local_slice(simg, band))      # RAW sums over this band's own rows
         m.set_band(False)
+        if not means:
+            return means, srms
         flat = torch.cat([t.flatten() for t in means + srms])
         self._group.all_reduce_sum(flat)
-        counts = D.tap_pixel_counts(sh, sw)
+        counts = D.tap_pixel_counts(sh, sw, m.style_layers)
         out, off = [], 0
         for t in means + srms:
             out.append(flat[off:off + t.numel()].view_as(t))
             off += t.numel()
-        means = [t / n for t, n in zip(out[:5], counts)]
-        srms = [t / n for t, n in zip(out[5:], counts)]
+        n = len(means)
+        means = [t / c for t, c in zip(out[:n], counts)]
+        srms = [t / c for t, c in zip(out[n:], counts)]
         return means, srms
 
     def _wait_loss(self, step):
@@ -710,16 +779,23 @@ class StyleTransfer:
                 t0 = time.perf_counter()
             elif time.perf_counter() - t0 > float(os.environ.get('STB_LOSS_TIMEOUT_S', '120')):
                 raise _lib.NativeError(f'iteration {step}: the device never published its loss (stamp {int(stamp[8])})')
-        return torch.from_numpy(self._ring_f32[slot, :8].copy())
+        # term k sits in word k below the stamp (word 8) and in word k + 1 above it
+        n = self.model.n_terms
+        words = self._ring_f32[slot, :8] if n <= 8 else np.concatenate([self._ring_f32[slot, :8],
+                                                                         self._ring_f32[slot, 9:n + 1]])
+        return torch.from_numpy(words[:n].copy())
 
     def loss_and_grad(self):
-        """Closure of ST:472-476 evaluated natively on the current image: returns (terms[8] host tensor, grad)."""
+        """Closure of ST:472-476 evaluated natively on the current image: returns (host tensor of the loss terms
+        [total, content terms, style terms, tv] of the layer table, grad)."""
         m = self.model
         grad = torch.empty_like(self.image)
         _lib.check(m.lib.stb_iterate_ex(m.ctx, _lib.ptr(self.image), None, None, None, 0, 0.0, 0.9, 0.99, 1e-8, 0.0, 0,
                                         _lib.ptr(grad), _lib.ptr(self._loss_host), _lib.cur_stream()))
         torch.cuda.current_stream().synchronize()
-        return self._loss_host.clone(), grad
+        if m.n_terms <= 8:
+            return self._loss_host[:m.n_terms].clone(), grad
+        return m.loss_terms(), grad
 
     # ------------------------------------------------------------------ the driver
     def stylize(self, content_image, style_images, *,
@@ -754,6 +830,10 @@ class StyleTransfer:
         (_Lockstep).  The first error of either rank stops both and is raised here, after rank 1's thread is joined and
         the whole image of the stopped iteration is back in self.average."""
         peer, shared = self._peer, self._group.shared
+        # rank 1 is an object of its own: it runs the layers set on this one
+        peer.content_layers = list(self.content_layers)
+        peer.style_layers = list(self.style_layers)
+        peer.style_weights = list(self.style_weights)
         if self._dev != peer._dev and not torch.cuda.can_device_access_peer(self._dev, peer._dev):
             return self._stylize_untiled(f'{self._dev} cannot access {peer._dev} peer to peer', content_image,
                                          style_images, callback, kw)
@@ -857,6 +937,15 @@ class StyleTransfer:
         if optimizer not in ('adam', 'lbfgs'):
             raise ValueError("optimizer must be one of 'adam', 'lbfgs'")
         per_content_weight = content_weight / len(self.content_layers)
+        # the layer attributes are read once per call (the reference re-reads them per scale): loss terms are
+        # zip(content_layers, content_weights) and zip(style_layers, style_weights) (ST:427, 451), so entries of
+        # style_layers without a weight, or weights without a layer, drop out
+        content_layers, style_layers = list(self.content_layers), list(self.style_layers)
+        check_layers(content_layers, style_layers)
+        layer_weights = [float(w) for w in self.style_weights][:len(style_layers)]
+        style_layers = style_layers[:len(layer_weights)]
+        content_weights = [per_content_weight] * len(content_layers)
+        self.model.set_layers(content_layers, style_layers)
 
         scales = gen_scales(min_scale, end_scale)
         cw, ch = size_to_fit(content_image.size, scales[0], scale_up=True)
@@ -930,7 +1019,7 @@ class StyleTransfer:
 
                 if self._verbose:
                     print(f'Processing content image ({cw}x{ch})...')
-                content_target = self.model.content_features(content)
+                content_targets = self.model.content_features_list(content)
                 means = srms = None
                 for weight, (sw, sh, simg) in zip(style_weights, styles):
                     if self._verbose:
@@ -946,8 +1035,8 @@ class StyleTransfer:
                             acc.add_(s * weight)
                 if band is not None:
                     self.model.set_band(True, ch, band.own0, band.own_rows)
-                self.model.set_targets(h_loc, cw, content_target, per_content_weight, means, srms, self.style_weights,
-                                       tv_weight)
+                self.model.set_targets_list(h_loc, cw, content_targets, content_weights, means, srms, layer_weights,
+                                            tv_weight)
                 if band is not None:
                     self._setup_comm(band, cw)
 
@@ -998,7 +1087,9 @@ class StyleTransfer:
                                 gpu_ram = max(gpu_ram, torch.cuda.max_memory_allocated(device))
                         if band is not None and self._comm_mode != 'peer':
                             torch.cuda.current_stream().synchronize()   # host-driven exchanges: plain read-back
-                            self.last_loss_terms = self._loss_host.clone()
+                            n = self.model.n_terms
+                            self.last_loss_terms = (self._loss_host[:n].clone() if n <= 8
+                                                    else self.model.loss_terms())
                         else:   # the reference syncs here (loss.item()); this waits for the loss only
                             self.last_loss_terms = self._wait_loss(step)
                         loss_value = float(self.last_loss_terms[0])
