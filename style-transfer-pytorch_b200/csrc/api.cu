@@ -9,6 +9,7 @@
 #include <cstring>
 #include <string>
 
+#include "comm.cuh"
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -425,11 +426,8 @@ __global__ void content_seed_kernel(const bf16* __restrict__ y, const bf16* __re
 __global__ void adam_rows_kernel(float* __restrict__ img, const float* __restrict__ grad, float* __restrict__ exp_avg,
                                  float* __restrict__ exp_avg_sq, float* __restrict__ ema, int H, int W, int row0,
                                  int rows, AdamScalars ac) {
-  const long per = (long)rows * W;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < 3 * per; i += (long)gridDim.x * blockDim.x) {
-    const int c = (int)(i / per);
-    const long r = i - (long)c * per;
-    const size_t idx = ((size_t)c * H + row0) * W + r;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * rows * W; i += gridDim.x * blockDim.x) {
+    const long idx = row_pos<1>(i, rows, W, H, row0).off;
     const float g = grad[idx];
     float m = exp_avg[idx], v = exp_avg_sq[idx], p = img[idx], e = ema[idx];
     adam_element(ac, g, m, v, p, e);
@@ -1207,6 +1205,7 @@ int stb_adam_update(float* img, const float* grad, float* exp_avg, float* exp_av
                     float ema_decay, void* stream) {
   STB_CHECK(img && grad && exp_avg && exp_avg_sq && ema, STB_ERR_INVALID, "null argument");
   STB_CHECK(row0 >= 0 && rows > 0 && row0 + rows <= H && step >= 1, STB_ERR_INVALID, "bad row range / step");
+  STB_CHECK(3l * rows * W < (1l << 31), STB_ERR_INVALID, "band of %d x %d pixels is too large", rows, W);
   const AdamScalars as = make_adam_scalars(step, lr, beta1, beta2, adam_eps, ema_decay);
   const long n = 3l * rows * W;
   long blocks = (n + 255) / 256;
@@ -1483,6 +1482,8 @@ int stb_comm_set_geometry(stb_ctx* ctx, int W, int h_local, int own0, int own_ro
                 h_local == own0 + own_rows + (has_dn ? COMM_APRON : 0), STB_ERR_INVALID,
             "band geometry: h_local=%d own0=%d own_rows=%d (aprons are %d rows)", h_local, own0, own_rows, COMM_APRON);
   if (has_up) STB_CHECK(up_apron_row0 + COMM_APRON == up_h_local, STB_ERR_INVALID, "upper neighbour geometry");
+  // the row kernels of the exchange walk a band with 32-bit indices
+  STB_CHECK(3l * h_local * W < (1l << 31), STB_ERR_INVALID, "band of %d x %d pixels is too large", h_local, W);
   ctx->comm.W = W; ctx->comm.h_local = h_local; ctx->comm.own0 = own0; ctx->comm.own_rows = own_rows;
   ctx->comm.up_h_local = up_h_local; ctx->comm.up_apron_row0 = up_apron_row0; ctx->comm.dn_h_local = dn_h_local;
   // halo_rows = 1: own rows only + one boundary-row pull per layer (needs the peer-mapped workspace); 0: recomputed aprons

@@ -32,16 +32,6 @@ namespace stb {
 
 namespace {
 
-// Row-wise kernels run on float4 when the image width is a multiple of 4 (rows are then 16-byte aligned) and on
-// scalars otherwise (odd pyramid widths such as 181 or 543).
-template <int V> struct Vec;
-template <> struct Vec<4> { typedef float4 T; };
-template <> struct Vec<1> { typedef float T; };
-__device__ __forceinline__ void unpack(const float4& v, float (&a)[4]) { a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w; }
-__device__ __forceinline__ void unpack(const float& v, float (&a)[1]) { a[0] = v; }
-__device__ __forceinline__ void pack(float4& v, const float (&a)[4]) { v = make_float4(a[0], a[1], a[2], a[3]); }
-__device__ __forceinline__ void pack(float& v, const float (&a)[1]) { v = a[0]; }
-
 // phase 0 BEGIN : t = ++iter;                     wait halo  stamps of the neighbours >= t - 1
 // phase 1 STATS : publish stats stamp = t;        wait stats stamps of ALL ranks      >= t
 // phase 2 GRAD  : publish grad  stamp = t;        wait grad  stamps of the neighbours >= t
@@ -71,25 +61,18 @@ __global__ void comm_phase_kernel(CommDev c, int phase) {
 // then still holds the rows the host sliced out of the full image)
 template <int V>
 __global__ void __launch_bounds__(256) halo_pull_kernel(CommDev c, float* __restrict__ img) {
-  typedef typename Vec<V>::T T;
   const unsigned long long t = reinterpret_cast<const unsigned long long*>(c.mbox[c.rank])[COMM_ITER];
   if (t <= 1) return;
-  const int w4 = c.W / V;
-  const long per_side = 3l * COMM_APRON * w4;
+  const int per_side = 3 * COMM_APRON * (c.W / V);
   const int sides = (c.rank > 0 ? 1 : 0) + (c.rank + 1 < c.world ? 1 : 0);
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < per_side * sides; i += (long)gridDim.x * blockDim.x) {
-    int side = (int)(i / per_side);           // 0: from the upper neighbour, 1: from the lower one
-    const long e = i - side * per_side;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < per_side * sides; i += gridDim.x * blockDim.x) {
+    int side = i / per_side;           // 0: from the upper neighbour, 1: from the lower one
+    const int e = i - side * per_side;
     if (c.rank == 0) side = 1;
-    const int ch = (int)(e / ((long)COMM_APRON * w4));
-    const long r4 = e - (long)ch * COMM_APRON * w4;
-    const int row = (int)(r4 / w4), x4 = (int)(r4 - (long)row * w4);
+    const RowPos p = row_pos<V>(e, COMM_APRON, c.W, c.h_local, side == 0 ? 0 : c.own0 + c.own_rows);
     // upper neighbour's LAST own rows = its outbox 1; lower neighbour's FIRST own rows = its outbox 0
-    const uint8_t* peer = c.mbox[side == 0 ? c.rank - 1 : c.rank + 1];
-    const T* src = reinterpret_cast<const T*>(peer + c.off_outbox[side == 0 ? 1 : 0]) +
-                   ((long)ch * COMM_APRON + row) * w4 + x4;
-    const int dst_row = side == 0 ? row : c.own0 + c.own_rows + row;
-    reinterpret_cast<T*>(img)[((long)ch * c.h_local + dst_row) * w4 + x4] = ld_peer(src);
+    const float* src = outbox_at(c, side == 0 ? c.rank - 1 : c.rank + 1, side == 0 ? 1 : 0, p.ch, p.r, p.x);
+    st<V>(img, p.off, ld_peer<V>(src, 0));
   }
 }
 
@@ -120,8 +103,6 @@ __global__ void __launch_bounds__(256) stats_allreduce_kernel(CommDev c, float* 
   }
 }
 
-// own rows: g = grad_local (+ upper neighbour's bottom-apron rows) (+ lower neighbour's top-apron rows); Adam; clamp;
-// EMA; the first / last APRON updated rows also go to the outboxes (the neighbours' next halo)
 // Per-layer halo exchange (DESIGN.md section 6, "halo mode"): the band computed only its own rows of a tensor; the one
 // row above / below them that the next 3x3 kernel reads is the neighbour's boundary own row, pulled here.  One kernel =
 // publish my progress stamp (everything before it on this stream is done: kernel boundary + system fence), wait for the
@@ -160,84 +141,38 @@ __global__ void __launch_bounds__(256) halo_rows_kernel(CommDev c, HaloRowArgs a
   }
 }
 
+// own rows: seam_gradient; Adam; clamp; EMA; the first / last APRON updated rows also go to the outboxes (the
+// neighbours' next halo).  add_seams = 0 (per-layer-halo mode): the local gradient of the own rows is already complete.
 template <int V>
 __global__ void __launch_bounds__(256)
 adam_seam_kernel(CommDev c, float* __restrict__ img, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                  float* __restrict__ ema, const AdamScalars* __restrict__ d_adam, int add_seams) {
-  typedef typename Vec<V>::T T;
   const AdamScalars ac = *d_adam;
-  const int w4 = c.W / V;
-  const long per = (long)c.own_rows * w4;
-  const T* grad = reinterpret_cast<const T*>(c.mbox[c.rank] + c.off_grad);
-  // add_seams = 0 (per-layer-halo mode): the local gradient of the own rows is already complete
-  const bool has_up = c.rank > 0 && add_seams, has_dn = c.rank + 1 < c.world && add_seams;
-  const T* gup = has_up ? reinterpret_cast<const T*>(c.mbox[c.rank - 1] + c.off_grad) : nullptr;
-  const T* gdn = has_dn ? reinterpret_cast<const T*>(c.mbox[c.rank + 1] + c.off_grad) : nullptr;
-  T* out_first = reinterpret_cast<T*>(c.mbox[c.rank] + c.off_outbox[0]);
-  T* out_last = reinterpret_cast<T*>(c.mbox[c.rank] + c.off_outbox[1]);
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < 3 * per; i += (long)gridDim.x * blockDim.x) {
-    const int ch = (int)(i / per);
-    const long r4 = i - (long)ch * per;
-    const int r = (int)(r4 / w4), x4 = (int)(r4 - (long)r * w4);
-    const long idx = ((long)ch * c.h_local + c.own0 + r) * w4 + x4;
-    float gg[V], aa[V], mm[V], vv[V], pp[V], ee[V];
-    unpack(grad[idx], gg);
-    if (has_up && r < COMM_APRON) {   // the upper band's bottom apron starts at its local row own0 + own_rows
-      unpack(ld_peer(gup + ((long)ch * c.up_h_local + c.up_apron_row0 + r) * w4 + x4), aa);
+  const int n = 3 * c.own_rows * (c.W / V);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const RowPos p = row_pos<V>(i, c.own_rows, c.W, c.h_local, c.own0);
+    Vec<V> g;
+    seam_gradient<V>(c, p.ch, p.r, p.x, add_seams, g);
+    Vec<V> m = ld<V>(exp_avg, p.off), v = ld<V>(exp_avg_sq, p.off), x = ld<V>(img, p.off), e = ld<V>(ema, p.off);
 #pragma unroll
-      for (int k = 0; k < V; ++k) gg[k] += aa[k];
-    }
-    if (has_dn && r >= c.own_rows - COMM_APRON) {   // the lower band's top apron is its local rows [0, APRON)
-      unpack(ld_peer(gdn + ((long)ch * c.dn_h_local + (r - (c.own_rows - COMM_APRON))) * w4 + x4), aa);
-#pragma unroll
-      for (int k = 0; k < V; ++k) gg[k] += aa[k];
-    }
-    unpack(reinterpret_cast<T*>(exp_avg)[idx], mm);
-    unpack(reinterpret_cast<T*>(exp_avg_sq)[idx], vv);
-    unpack(reinterpret_cast<T*>(img)[idx], pp);
-    unpack(reinterpret_cast<T*>(ema)[idx], ee);
-#pragma unroll
-    for (int k = 0; k < V; ++k) adam_element(ac, gg[k], mm[k], vv[k], pp[k], ee[k]);
-    T pn;
-    pack(pn, pp);
-    pack(reinterpret_cast<T*>(exp_avg)[idx], mm);
-    pack(reinterpret_cast<T*>(exp_avg_sq)[idx], vv);
-    reinterpret_cast<T*>(img)[idx] = pn;
-    pack(reinterpret_cast<T*>(ema)[idx], ee);
-    if (r < COMM_APRON) out_first[((long)ch * COMM_APRON + r) * w4 + x4] = pn;
-    if (r >= c.own_rows - COMM_APRON)
-      out_last[((long)ch * COMM_APRON + (r - (c.own_rows - COMM_APRON))) * w4 + x4] = pn;
+    for (int k = 0; k < V; ++k) adam_element(ac, g.v[k], m.v[k], v.v[k], x.v[k], e.v[k]);
+    st<V>(exp_avg, p.off, m);
+    st<V>(exp_avg_sq, p.off, v);
+    st<V>(img, p.off, x);
+    outbox_store<V>(c, p.ch, p.r, p.x, x);
+    st<V>(ema, p.off, e);
   }
 }
 
-// banded L-BFGS: g[3][own_rows][W] (compact) = the own rows of the local gradient (+ the neighbours' apron rows), summed
-// in the order of adam_seam_kernel: own, upper, lower
+// banded L-BFGS: g[3][own_rows][W] (compact) = seam_gradient of the own rows
 template <int V>
 __global__ void __launch_bounds__(256) lbfgs_seam_gather_kernel(CommDev c, float* __restrict__ g, int add_seams) {
-  typedef typename Vec<V>::T T;
-  const int w4 = c.W / V;
-  const long per = (long)c.own_rows * w4;
-  const T* grad = reinterpret_cast<const T*>(c.mbox[c.rank] + c.off_grad);
-  const bool has_up = c.rank > 0 && add_seams, has_dn = c.rank + 1 < c.world && add_seams;
-  const T* gup = has_up ? reinterpret_cast<const T*>(c.mbox[c.rank - 1] + c.off_grad) : nullptr;
-  const T* gdn = has_dn ? reinterpret_cast<const T*>(c.mbox[c.rank + 1] + c.off_grad) : nullptr;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < 3 * per; i += (long)gridDim.x * blockDim.x) {
-    const int ch = (int)(i / per);
-    const long r4 = i - (long)ch * per;
-    const int r = (int)(r4 / w4), x4 = (int)(r4 - (long)r * w4);
-    float gg[V], aa[V];
-    unpack(grad[((long)ch * c.h_local + c.own0 + r) * w4 + x4], gg);
-    if (has_up && r < COMM_APRON) {
-      unpack(ld_peer(gup + ((long)ch * c.up_h_local + c.up_apron_row0 + r) * w4 + x4), aa);
-#pragma unroll
-      for (int k = 0; k < V; ++k) gg[k] += aa[k];
-    }
-    if (has_dn && r >= c.own_rows - COMM_APRON) {
-      unpack(ld_peer(gdn + ((long)ch * c.dn_h_local + (r - (c.own_rows - COMM_APRON))) * w4 + x4), aa);
-#pragma unroll
-      for (int k = 0; k < V; ++k) gg[k] += aa[k];
-    }
-    pack(reinterpret_cast<T*>(g)[i], gg);
+  const int n = 3 * c.own_rows * (c.W / V);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const RowPos p = row_pos<V>(i, c.own_rows, c.W, c.h_local, c.own0);
+    Vec<V> gv;
+    seam_gradient<V>(c, p.ch, p.r, p.x, add_seams, gv);
+    st<V>(g, (long)i * V, gv);
   }
 }
 
@@ -285,8 +220,9 @@ int launch_comm_phase(const CommDev& c, int phase, cudaStream_t s) {
 
 int launch_halo_pull(const CommDev& c, float* img, cudaStream_t s) {
   if (c.world <= 1) return STB_OK;
-  if (c.W % 4 == 0) halo_pull_kernel<4><<<grid_for(6l * COMM_APRON * (c.W / 4)), 256, 0, s>>>(c, img);
-  else halo_pull_kernel<1><<<grid_for(6l * COMM_APRON * c.W), 256, 0, s>>>(c, img);
+  with_row_vec(c.W, 6l * COMM_APRON, [&](auto v, long n) {
+    halo_pull_kernel<decltype(v)::value><<<grid_for(n), 256, 0, s>>>(c, img);
+  });
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
 }
@@ -321,21 +257,18 @@ int launch_halo_rows(const CommDev& c, const HaloRowArgs& a, cudaStream_t s) {
 
 int launch_adam_seam(const CommDev& c, float* img, float* exp_avg, float* exp_avg_sq, float* ema,
                      const AdamScalars* d_adam, int add_seams, cudaStream_t s) {
-  if (c.W % 4 == 0)
-    adam_seam_kernel<4><<<grid_for(3l * c.own_rows * (c.W / 4)), 256, 0, s>>>(c, img, exp_avg, exp_avg_sq, ema, d_adam,
-                                                                             add_seams);
-  else
-    adam_seam_kernel<1><<<grid_for(3l * c.own_rows * c.W), 256, 0, s>>>(c, img, exp_avg, exp_avg_sq, ema, d_adam,
-                                                                        add_seams);
+  with_row_vec(c.W, 3l * c.own_rows, [&](auto v, long n) {
+    adam_seam_kernel<decltype(v)::value><<<grid_for(n), 256, 0, s>>>(c, img, exp_avg, exp_avg_sq, ema, d_adam,
+                                                                      add_seams);
+  });
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
 }
 
 int launch_lbfgs_seam_gather(const CommDev& c, float* g, int add_seams, cudaStream_t s) {
-  if (c.W % 4 == 0)
-    lbfgs_seam_gather_kernel<4><<<grid_for(3l * c.own_rows * (c.W / 4)), 256, 0, s>>>(c, g, add_seams);
-  else
-    lbfgs_seam_gather_kernel<1><<<grid_for(3l * c.own_rows * c.W), 256, 0, s>>>(c, g, add_seams);
+  with_row_vec(c.W, 3l * c.own_rows, [&](auto v, long n) {
+    lbfgs_seam_gather_kernel<decltype(v)::value><<<grid_for(n), 256, 0, s>>>(c, g, add_seams);
+  });
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
 }

@@ -123,25 +123,6 @@ __device__ __forceinline__ double reduce_partials(const double* p, int nb, doubl
   return block_reduce<kMax>(v, sm);
 }
 
-// L consecutive floats at j (L = 4: one 16-byte access; the vectors and the caller's tensors are 16-byte aligned)
-template <int L> struct Vec { float v[L]; };
-template <int L>
-__device__ __forceinline__ Vec<L> ld(const float* p, long j) {
-  Vec<L> r;
-  if constexpr (L == 4) {
-    const float4 t = *reinterpret_cast<const float4*>(p + j);
-    r.v[0] = t.x; r.v[1] = t.y; r.v[2] = t.z; r.v[3] = t.w;
-  } else {
-    r.v[0] = p[j];
-  }
-  return r;
-}
-template <int L>
-__device__ __forceinline__ void st(float* p, long j, const Vec<L>& r) {
-  if constexpr (L == 4) *reinterpret_cast<float4*>(p + j) = make_float4(r.v[0], r.v[1], r.v[2], r.v[3]);
-  else p[j] = r.v[0];
-}
-
 // calls body(Vec-width constant, j) over [0, n): 4-wide chunks in a grid-stride loop, then the < 4 scalar tail
 template <typename Body>
 __device__ __forceinline__ void for_each(long n, Body&& body) {
@@ -392,7 +373,7 @@ static_assert(COMM_XVAL + 2 * LBFGS_XREDUCES * 4 <= 4096 / 8, "cross-rank values
 static_assert(LBFGS_XREDUCES < 32, "stamp = iteration * 32 + seq");
 
 // final pass of the banded step on the own rows of the local image; the first / last COMM_APRON rows also go to the
-// outboxes (the neighbours' next halo), as adam_seam_kernel does
+// outboxes (the neighbours' next halo)
 template <int V>
 __global__ void __launch_bounds__(LB_THREADS) lbfgs_final_banded_kernel(LbState s, CommDev c, float* __restrict__ x,
                                                                         float* __restrict__ ema, float decay) {
@@ -400,20 +381,12 @@ __global__ void __launch_bounds__(LB_THREADS) lbfgs_final_banded_kernel(LbState 
   const bool skip = s.hdr->skip != 0;
   const bool take = final_take(s, 1, sm);
   const float t = s.hdr->t;
-  const int wv = c.W / V;
-  const int per = c.own_rows * wv;   // 3 * per < 2^31 (launch_lbfgs_step_banded)
-  float* out_first = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_outbox[0]);
-  float* out_last = reinterpret_cast<float*>(c.mbox[c.rank] + c.off_outbox[1]);
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * per; i += gridDim.x * blockDim.x) {
-    const int ch = i / per;
-    const int r4 = i - ch * per;
-    const int r = r4 / wv;
-    const long xo = (long)(r4 - r * wv) * V;
+  const int n = 3 * c.own_rows * (c.W / V);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const RowPos p = row_pos<V>(i, c.own_rows, c.W, c.h_local, c.own0);
     Vec<V> xv;
-    final_elems<V>(s, take, skip, t, decay, x, ema, ((long)ch * c.h_local + c.own0 + r) * c.W + xo, (long)i * V, xv);
-    if (r < COMM_APRON) st<V>(out_first, ((long)ch * COMM_APRON + r) * c.W + xo, xv);
-    if (r >= c.own_rows - COMM_APRON)
-      st<V>(out_last, ((long)ch * COMM_APRON + (r - (c.own_rows - COMM_APRON))) * c.W + xo, xv);
+    final_elems<V>(s, take, skip, t, decay, x, ema, p.off, (long)i * V, xv);
+    outbox_store<V>(c, p.ch, p.r, p.x, xv);
   }
 }
 
@@ -455,8 +428,9 @@ int launch_lbfgs_step_banded(void* state, const CommDev& c, float* x, float* ema
     lbfgs_round_kernel<<<nb, LB_THREADS, 0, s>>>(st, r, 1);
     lbfgs_xreduce_kernel<<<1, LB_THREADS, 0, s>>>(c, st.part + (r & 1) * LB_MAX_BLOCKS, 1, nb, 0, r + 1);
   }
-  if (c.W % 4 == 0) lbfgs_final_banded_kernel<4><<<nb, LB_THREADS, 0, s>>>(st, c, x, ema, ema_decay);
-  else lbfgs_final_banded_kernel<1><<<nb, LB_THREADS, 0, s>>>(st, c, x, ema, ema_decay);
+  with_row_vec(c.W, 3l * c.own_rows, [&](auto v, long) {
+    lbfgs_final_banded_kernel<decltype(v)::value><<<nb, LB_THREADS, 0, s>>>(st, c, x, ema, ema_decay);
+  });
   STB_CUDA_CHECK(cudaGetLastError());
   return STB_OK;
 }
