@@ -167,6 +167,15 @@ STB_API int stb_set_loss_ring(stb_ctx* ctx, float* host_ring, int slots);
 STB_API int stb_resize(const float* in, int C, int H, int W, float* out, int Ho, int Wo, int mode, int post,
                        void* stream);
 
+/* ------------------------------------------------------------------ image snapshot (get_image, periodic saves)
+ * value: planar fp32 [3][H][W] (the EMA's storage); out: interleaved [H][W][3], written in one pass on `stream`.
+ *   kind 0: uint8  = trunc(clamp(value / denom, 0, 1) * 255)       (to_pil_image: mul(255).byte())
+ *   kind 1: uint16 = round_half_even(clamp(value / denom, 0, 1) * 65535)   (np.uint16(np.round(x * 65535)))
+ * The division is a multiply by 1 / denom, computed in double and rounded to float, as torch computes
+ * `tensor / python_float` on CUDA, so the result is bit-identical to those expressions on EMA.get().  denom = 1 - accum, or 1 for an image that is already
+ * bias-corrected.  STB_ERR_INVALID for null pointers, H or W < 1, or a kind other than 0 and 1. */
+STB_API int stb_snapshot(const float* value, int H, int W, double denom, int kind, void* out, void* stream);
+
 /* ------------------------------------------------------------------ tiled iteration, exchanges inside the library
  * (csrc/comm.cu).  Each rank owns a MAILBOX (iteration stamps, its statistics block, its image gradient, its first /
  * last 80 updated rows) that the peers map with CUDA IPC and read over NVLink; stb_iterate_banded is then the whole

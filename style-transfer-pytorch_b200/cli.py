@@ -3,8 +3,10 @@
 Same flags as the reference CLI (/root/reference/style_transfer/cli.py:155-203): positional content + styles,
 `-o/--output`, `-sw/--style-weights`, `-d/--devices`, `-r/--random-seed`, `-p/--pooling`, `--save-every`, and one
 option per keyword of `StyleTransfer.stylize` whose default and type are read from the method's signature (as
-CLI:150-153 does).  Out of scope here (SURVEY.md section 2, rows 16-19): ICC colour management / soft proofing,
-16-bit TIFF output and the web monitor; `--web`, `--proof` and `.tif` outputs exit with a clear message.
+CLI:150-153 does).  Image I/O follows the reference too: inputs with an embedded ICC profile are converted to sRGB,
+`--proof PROFILE` soft-proofs the content and style images through a CMYK profile, and a `.tif`/`.tiff` output is
+written with 16 bits per channel and an sRGB profile (image_io.py).  Out of scope (SURVEY.md section 2, row 18): the web
+monitor; `--web` exits with a clear message.
 """
 from __future__ import annotations
 
@@ -16,22 +18,14 @@ from dataclasses import asdict
 from pathlib import Path
 
 import torch
-from PIL import Image
 
-from .image_io import AsyncImageWriter
+from .image_io import TIFF_SUFFIXES, AsyncImageWriter, load_image, srgb_profile, write_tiff16
 from .style_transfer import StyleTransfer
 
 _SHORT = {'content_weight': 'cw', 'tv_weight': 'tw', 'optimizer': None, 'min_scale': 'ms', 'end_scale': 's',
           'iterations': 'i', 'initial_iterations': 'ii', 'step_size': 'ss', 'avg_decay': 'ad', 'init': None,
           'style_scale_fac': 'ssf', 'style_size': 'sz'}
 _CHOICES = {'optimizer': ['adam', 'lbfgs'], 'init': ['content', 'gray', 'uniform', 'normal', 'style_stats']}
-
-
-def _read_rgb(path):
-    try:
-        return Image.open(path).convert('RGB')
-    except OSError as err:
-        sys.exit(f'{type(err).__name__}: {err}')
 
 
 def build_parser():
@@ -47,7 +41,8 @@ def build_parser():
                     help="the model's pooling mode")
     ap.add_argument('--save-every', type=int, default=0, help='save the image every SAVE_EVERY iterations')
     ap.add_argument('--web', default=False, action='store_true', help='(not supported in this build)')
-    ap.add_argument('--proof', type=str, default=None, help='(not supported in this build)')
+    ap.add_argument('--proof', type=str, default=None, metavar='PROFILE',
+                    help='soft-proof the content and style images through this CMYK ICC profile')
     defaults = StyleTransfer.stylize.__kwdefaults__
     types = StyleTransfer.stylize.__annotations__
     for name, short in _SHORT.items():
@@ -62,13 +57,12 @@ def build_parser():
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
-    if args.web or args.proof:
-        sys.exit('--web / --proof are outside the scope of the H100-native hot-path build')
+    if args.web:
+        sys.exit('--web is outside the scope of the H100-native hot-path build')
     out_path = Path(args.output)
-    if out_path.suffix.lower() in ('.tif', '.tiff'):
-        sys.exit('16-bit TIFF output is outside the scope of this build; use .png/.jpg/.webp')
-    content = _read_rgb(args.content)
-    styles = [_read_rgb(p) for p in args.styles]
+    tiff = out_path.suffix.lower() in TIFF_SUFFIXES   # 16 bits per channel, sRGB-tagged (reference CLI:63-81)
+    content = load_image(args.content, args.proof)
+    styles = [load_image(p, args.proof) for p in args.styles]
 
     # one process per GPU under torchrun: the ranks tile the large scales between them (distributed.py); rank 0 talks
     # and writes, every rank takes part in the collective gathers behind get_image()
@@ -124,12 +118,15 @@ def main(argv=None):
     except KeyboardInterrupt:
         pass
     writer.close()
-    image = st.get_image()
+    image = st.get_image('np_uint16' if tiff else 'pil')
     if rank != 0:
         return
     if image is not None:
         print(f'Writing image to {out_path}.')
-        image.save(out_path)
+        if tiff:
+            write_tiff16(out_path, image, srgb_profile)
+        else:
+            image.save(out_path)
     with open('trace.json', 'w') as fp:
         json.dump(dict(args={k: (str(v) if isinstance(v, Path) else v) for k, v in vars(args).items()},
                        iterates=trace), fp, indent=4)

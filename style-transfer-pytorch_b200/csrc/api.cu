@@ -1223,6 +1223,12 @@ int stb_resize(const float* in, int C, int H, int W, float* out, int Ho, int Wo,
   return launch_resize(in, C, H, W, out, Ho, Wo, mode, post, static_cast<cudaStream_t>(stream));
 }
 
+// Device snapshot of the averaged image for saving (get_image, AsyncImageWriter): one pass from the EMA's planar
+// storage to interleaved uint8 / uint16, outside every iteration graph.
+int stb_snapshot(const float* value, int H, int W, double denom, int kind, void* out, void* stream) {
+  return launch_snapshot(value, H, W, denom, kind, out, static_cast<cudaStream_t>(stream));
+}
+
 int stb_iterate(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step, float lr,
                 float beta1, float beta2, float adam_eps, float ema_decay, float* loss_out_host8, void* stream) {
   return stb_iterate_ex(ctx, img, exp_avg, exp_avg_sq, ema, step, lr, beta1, beta2, adam_eps, ema_decay, 1, nullptr,

@@ -482,12 +482,103 @@ int launch_resize(const float* in, int C, int H, int W, float* out, int Ho, int 
   return STB_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ image snapshot
+// The averaged image as the host saves it: planar fp32 [3][H][W] EMA storage in, interleaved [H][W][3] out, in one pass.
+//   KIND 0: uint8  = trunc(clamp(v * inv, 0, 1) * 255)          (get_image('pil'): to_pil_image's mul(255).byte())
+//   KIND 1: uint16 = rint(clamp(v * inv, 0, 1) * 65535)         (get_image('np_uint16'): np.round(x * 65535))
+// inv = 1 / (1 - accum) computed in double on the host and rounded to float: torch evaluates `tensor / python_float` on
+// CUDA as a multiply by that reciprocal.  The _rn intrinsics keep nvcc from contracting the two multiplies into an FMA; the clamp is written
+// with comparisons so that a NaN passes through it as it does through torch.clamp (and then converts to 0).
+template <int KIND>
+__device__ __forceinline__ uint32_t snap_quant(float v, float inv) {
+  float x = __fmul_rn(v, inv);
+  x = x < 0.f ? 0.f : (x > 1.f ? 1.f : x);
+  if (KIND == 0) return __float2uint_rz(__fmul_rn(x, 255.f));
+  return __float2uint_rz(rintf(__fmul_rn(x, 65535.f)));
+}
+
+// One thread = 8 consecutive pixels: two float4 loads per plane, then 24 output values stored as three 8-byte (uint8)
+// or three 16-byte (uint16) words.  VEC needs hw % 4 == 0 (so that every plane starts 16-byte aligned) and 16-byte
+// aligned pointers; otherwise, and for the ragged last group, pixels are loaded and stored one element at a time.
+constexpr int SNAP_PIX = 8;
+
+template <int KIND, bool VEC>
+__global__ void __launch_bounds__(256)
+snapshot_kernel(const float* __restrict__ v, int hw, float inv, void* __restrict__ out) {
+  using T = typename std::conditional<KIND == 0, uint8_t, uint16_t>::type;
+  constexpr int BITS = 8 * sizeof(T);
+  const int groups = (hw + SNAP_PIX - 1) / SNAP_PIX;
+  for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += gridDim.x * blockDim.x) {
+    const int p0 = g * SNAP_PIX;
+    T* __restrict__ o = reinterpret_cast<T*>(out) + (size_t)p0 * 3;
+    if (VEC && p0 + SNAP_PIX <= hw) {
+      float px[3][SNAP_PIX];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float4* src = reinterpret_cast<const float4*>(v + (size_t)c * hw + p0);
+        const float4 a = __ldg(src), b = __ldg(src + 1);
+        px[c][0] = a.x; px[c][1] = a.y; px[c][2] = a.z; px[c][3] = a.w;
+        px[c][4] = b.x; px[c][5] = b.y; px[c][6] = b.z; px[c][7] = b.w;
+      }
+      // HWC element e = 3 * pixel + channel, packed little-endian into 32-bit words
+      constexpr int PER_WORD = 32 / BITS, WORDS = 3 * SNAP_PIX / PER_WORD;
+      uint32_t w[WORDS];
+#pragma unroll
+      for (int i = 0; i < WORDS; ++i) {
+        w[i] = 0u;
+#pragma unroll
+        for (int j = 0; j < PER_WORD; ++j) {
+          const int e = i * PER_WORD + j;
+          w[i] |= snap_quant<KIND>(px[e % 3][e / 3], inv) << (BITS * j);
+        }
+      }
+      if (KIND == 0) {
+        uint2* d = reinterpret_cast<uint2*>(o);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) d[i] = make_uint2(w[2 * i], w[2 * i + 1]);
+      } else {
+        uint4* d = reinterpret_cast<uint4*>(o);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) d[i] = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
+      }
+    } else {
+      const int n = min(SNAP_PIX, hw - p0);
+      for (int k = 0; k < n; ++k)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) o[3 * k + c] = (T)snap_quant<KIND>(__ldg(v + (size_t)c * hw + p0 + k), inv);
+    }
+  }
+}
+
+int launch_snapshot(const float* value, int H, int W, double denom, int kind, void* out, cudaStream_t s) {
+  STB_CHECK(value && out, STB_ERR_INVALID, "snapshot: null pointer");
+  STB_CHECK(H >= 1 && W >= 1, STB_ERR_INVALID, "snapshot: bad shape %d x %d", H, W);
+  STB_CHECK(kind == 0 || kind == 1, STB_ERR_INVALID, "snapshot: unknown kind %d", kind);
+  STB_CHECK((long)H * W <= (1l << 31) - SNAP_PIX, STB_ERR_INVALID, "snapshot: %d x %d pixels is too large", H, W);
+  const int hw = H * W;
+  const float inv = (float)(1.0 / denom);   // as torch forms it for a CPU scalar divisor (checked bit for bit)
+  const bool vec = hw % 4 == 0 && reinterpret_cast<uintptr_t>(value) % 16 == 0 &&
+                   reinterpret_cast<uintptr_t>(out) % 16 == 0;
+  const int g = grid_for((hw + SNAP_PIX - 1) / SNAP_PIX, 256);
+  if (kind == 0) {
+    if (vec) snapshot_kernel<0, true><<<g, 256, 0, s>>>(value, hw, inv, out);
+    else snapshot_kernel<0, false><<<g, 256, 0, s>>>(value, hw, inv, out);
+  } else {
+    if (vec) snapshot_kernel<1, true><<<g, 256, 0, s>>>(value, hw, inv, out);
+    else snapshot_kernel<1, false><<<g, 256, 0, s>>>(value, hw, inv, out);
+  }
+  STB_CUDA_CHECK(cudaGetLastError());
+  return STB_OK;
+}
+
 int preload_image_kernels() {
   cudaFuncAttributes fa;
 #define STB_PRELOAD(k) STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(k)))
   STB_PRELOAD(tv_kernel); STB_PRELOAD(pack_w0_fwd_kernel); STB_PRELOAD(conv0_bwd_adam_kernel);
   STB_PRELOAD(pool_bwd_kernel<STB_POOL_MAX>); STB_PRELOAD(pool_bwd_kernel<STB_POOL_AVERAGE>);
   STB_PRELOAD(pool_bwd_kernel<STB_POOL_L2>); STB_PRELOAD(sse_kernel); STB_PRELOAD(resize_kernel);
+  STB_PRELOAD((snapshot_kernel<0, true>)); STB_PRELOAD((snapshot_kernel<0, false>));
+  STB_PRELOAD((snapshot_kernel<1, true>)); STB_PRELOAD((snapshot_kernel<1, false>));
 #undef STB_PRELOAD
   return STB_OK;
 }

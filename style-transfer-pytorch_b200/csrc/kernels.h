@@ -96,6 +96,8 @@ int launch_sse(const bf16* a, const bf16* b, long n, float* partials, int* n_par
 // F.interpolate(align_corners=False) on fp32 [C][H][W] planes: mode 0 bilinear / 1 bicubic; post 0 none / 1 relu /
 // 2 clamp to [0,1]  (warm start of a scale, ST:285-295, 420)
 int launch_resize(const float* in, int C, int H, int W, float* out, int Ho, int Wo, int mode, int post, cudaStream_t s);
+// fp32 [3][H][W] / denom, clamped to [0,1], quantised to interleaved [H][W][3]: kind 0 uint8, 1 uint16 (stb_snapshot)
+int launch_snapshot(const float* value, int H, int W, double denom, int kind, void* out, cudaStream_t s);
 
 // ---------------------------------------------------------------- L-BFGS step on the device (lbfgs.cu)
 // torch.optim.LBFGS.step (lr 1, max_iter 1, history STB_LBFGS_HISTORY, no line search) + EMA on n-float vectors; the

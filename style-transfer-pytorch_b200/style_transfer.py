@@ -586,18 +586,35 @@ class StyleTransfer:
             value = D.gather_rows(value, self._band, self._group)
         return value[0].clamp(0, 1)
 
+    def _snapshot(self, kind):
+        """The averaged image quantised on the device by stb_snapshot, as an [H, W, 3] tensor ready on the current
+        stream: kind 0 uint8 (to_pil_image's mul(255).byte()), kind 1 uint16 (np.uint16(np.round(x * 65535))).
+
+        Untiled, the kernel reads the EMA's storage on the iteration stream, ordered after the iterations, with no host
+        synchronisation and no fp32 temporary.  On a banded scale the image is first gathered by get_image_tensor()
+        (collective), and the gathered image, already bias-corrected, is quantised with denom = 1."""
+        if self._band is not None:
+            src, denom = self.get_image_tensor(), 1.0
+        else:
+            src, denom = self.average.value, 1 - self.average.accum
+        h, w = src.shape[-2:]
+        cur = torch.cuda.current_stream(self._dev)
+        with torch.cuda.device(self._dev), torch.cuda.stream(self._stream):
+            self._stream.wait_stream(cur)
+            out = torch.empty(h, w, 3, dtype=(torch.uint8, torch.uint16)[kind], device=self._dev)
+            _lib.check(self.model.lib.stb_snapshot(_lib.ptr(src), h, w, denom, kind, _lib.ptr(out),
+                                                   _lib.cur_stream()))
+        cur.wait_stream(self._stream)
+        return out
+
     def get_image(self, image_type='pil'):
         if self.average is None:
             return None
-        image = self.get_image_tensor()
         kind = image_type.lower()
         if kind == 'pil':
-            # torchvision to_pil_image semantics (mul(255).byte()); made HWC-contiguous on the device so that the
-            # host side is a single 3-byte/pixel copy
-            arr = image.mul(255).byte().permute(1, 2, 0).contiguous().cpu().numpy()
-            return Image.fromarray(arr)
+            return Image.fromarray(self._snapshot(0).cpu().numpy())
         if kind == 'np_uint16':
-            return np.uint16(np.round(image.cpu().movedim(0, 2).numpy() * 65535))
+            return self._snapshot(1).cpu().numpy()
         raise ValueError("image_type must be 'pil' or 'np_uint16'")
 
     # ------------------------------------------------------------------ helpers
