@@ -5,8 +5,12 @@ Same flags as the reference CLI (/root/reference/style_transfer/cli.py:155-203):
 option per keyword of `StyleTransfer.stylize` whose default and type are read from the method's signature (as
 CLI:150-153 does).  Image I/O follows the reference too: inputs with an embedded ICC profile are converted to sRGB,
 `--proof PROFILE` soft-proofs the content and style images through a CMYK profile, and a `.tif`/`.tiff` output is
-written with 16 bits per channel and an sRGB profile (image_io.py).  Out of scope (SURVEY.md section 2, row 18): the web
-monitor; `--web` exits with a clear message.
+written with 16 bits per channel and an sRGB profile (image_io.py).
+
+`--web` serves the live monitor (web.py) at http://HOST:PORT/ (`--host`, default 0.0.0.0; `--port`, default 8080, 0 for
+any free port; `--browser [NAME]` opens it).  Rank 0 feeds it every iteration; its image is a device snapshot taken when
+a browser has fetched the previous one and at the end of every scale.  Under torchrun only rank 0 serves, and on a scale
+tiled across the ranks its image refreshes only where every rank gathers anyway: at the saves and the scale ends.
 """
 from __future__ import annotations
 
@@ -40,7 +44,11 @@ def build_parser():
     ap.add_argument('--pooling', '-p', type=str, default='max', choices=['max', 'average', 'l2'],
                     help="the model's pooling mode")
     ap.add_argument('--save-every', type=int, default=0, help='save the image every SAVE_EVERY iterations')
-    ap.add_argument('--web', default=False, action='store_true', help='(not supported in this build)')
+    ap.add_argument('--web', default=False, action='store_true', help='enable the live web monitor')
+    ap.add_argument('--host', type=str, default='0.0.0.0', help='the host the web monitor binds to')
+    ap.add_argument('--port', type=int, default=8080, help='the port the web monitor binds to (0: any free port)')
+    ap.add_argument('--browser', type=str, default='', nargs='?',
+                    help='open a web browser (name one if not the system default)')
     ap.add_argument('--proof', type=str, default=None, metavar='PROFILE',
                     help='soft-proof the content and style images through this CMYK ICC profile')
     defaults = StyleTransfer.stylize.__kwdefaults__
@@ -57,8 +65,6 @@ def build_parser():
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
-    if args.web:
-        sys.exit('--web is outside the scope of the H100-native hot-path build')
     out_path = Path(args.output)
     tiff = out_path.suffix.lower() in TIFF_SUFFIXES   # 16 bits per channel, sRGB-tagged (reference CLI:63-81)
     content = load_image(args.content, args.proof)
@@ -94,27 +100,61 @@ def main(argv=None):
     else:
         args.end_scale = int(end_scale)
 
+    web = None
+    if args.web and rank == 0:   # only rank 0 serves: the other ranks cannot see the browser's requests
+        from .web import WebInterface
+        web = WebInterface(args.host, args.port)
+    try:
+        _run(args, content, styles, devices, rank, out_path, tiff, web)
+    finally:
+        if web is not None:
+            web.close()
+
+
+def _run(args, content, styles, devices, rank, out_path, tiff, web):
     for device in devices:
         torch.tensor(0).to(device)
     torch.manual_seed(args.random_seed)
     st = StyleTransfer(devices=[str(d) for d in devices], pooling=args.pooling)
     trace = []
     writer = AsyncImageWriter()  # periodic saves are encoded off the loop's critical path (image_io.py)
+    if web is not None:
+        import webbrowser
+        if args.browser:
+            webbrowser.get(args.browser).open(web.url)
+        elif args.browser is None:
+            webbrowser.open(web.url)
+    done_after_run = []
 
     def on_iterate(it):
         trace.append(asdict(it))
         if rank == 0:
             print(f'Size: {it.w}x{it.h}, iteration: {it.i}, loss: {it.loss:g}')
         last_of_scale = it.i == it.i_max
-        if (args.save_every and it.i % args.save_every == 0) or (last_of_scale and max(it.w, it.h) != args.end_scale):
+        end = max(it.w, it.h) == args.end_scale
+        # a scale tiled across processes: a gather takes every rank, so the monitor's image comes from the saves' gathers
+        tiled_apart = web is not None and st._band is not None and st._sync is None
+        gathered = None
+        if (args.save_every and it.i % args.save_every == 0) or (last_of_scale and not end):
             if rank == 0:
-                writer.submit_snapshot(st, out_path)
+                if tiled_apart:
+                    gathered = st.get_image_tensor()
+                writer.submit_snapshot(st, out_path, gathered)
             else:
                 st.get_image_tensor()   # the gather of a tiled scale is collective
+        if web is not None:
+            web.put_iterate(it, st, gathered=gathered)
+            if last_of_scale and end:
+                if tiled_apart:
+                    done_after_run.append(True)   # the final image is whole once stylize() has stitched the bands
+                else:
+                    web.put_done()
 
     kwargs = {k: getattr(args, k) for k in _SHORT}
     try:
         st.stylize(content, styles, style_weights=args.style_weights, callback=on_iterate, **kwargs)
+        if done_after_run:
+            web.put_done(st)
     except KeyboardInterrupt:
         pass
     writer.close()

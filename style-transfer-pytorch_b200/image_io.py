@@ -145,12 +145,13 @@ class AsyncImageWriter:
         self._thread.start()
 
     # ------------------------------------------------------------------ producer side (the stylize callback)
-    def submit_snapshot(self, st, path):
+    def submit_snapshot(self, st, path, gathered=None):
         """Snapshot `st`'s current averaged image on the device and queue it for saving to `path`: 16 bits per channel
-        for `.tif`/`.tiff`, 8 otherwise.  On an untiled scale this does not wait for the device."""
+        for `.tif`/`.tiff`, 8 otherwise.  On an untiled scale this does not wait for the device.  `gathered`: the image
+        st.get_image_tensor() has already returned at this iteration, saved instead of gathering it again."""
         import torch
         path = Path(path)
-        snap = st._snapshot(1 if path.suffix.lower() in TIFF_SUFFIXES else 0)
+        snap = st._snapshot(1 if path.suffix.lower() in TIFF_SUFFIXES else 0, gathered)
         stream = st._stream
         host = torch.empty(snap.shape, dtype=snap.dtype, pin_memory=True)
         with torch.cuda.stream(stream):

@@ -586,14 +586,17 @@ class StyleTransfer:
             value = D.gather_rows(value, self._band, self._group)
         return value[0].clamp(0, 1)
 
-    def _snapshot(self, kind):
+    def _snapshot(self, kind, gathered=None):
         """The averaged image quantised on the device by stb_snapshot, as an [H, W, 3] tensor ready on the current
         stream: kind 0 uint8 (to_pil_image's mul(255).byte()), kind 1 uint16 (np.uint16(np.round(x * 65535))).
 
         Untiled, the kernel reads the EMA's storage on the iteration stream, ordered after the iterations, with no host
         synchronisation and no fp32 temporary.  On a banded scale the image is first gathered by get_image_tensor()
-        (collective), and the gathered image, already bias-corrected, is quantised with denom = 1."""
-        if self._band is not None:
+        (collective), and the gathered image, already bias-corrected, is quantised with denom = 1.  `gathered`: an
+        image get_image_tensor() has already returned at this iteration, quantised instead of gathering again."""
+        if gathered is not None:
+            src, denom = gathered, 1.0
+        elif self._band is not None:
             src, denom = self.get_image_tensor(), 1.0
         else:
             src, denom = self.average.value, 1 - self.average.accum
