@@ -15,15 +15,16 @@ product with cscale and the last sum are four more roundings of values bounded b
 So |v - ref| <= delta = 2 u (K + 4) (M + |gmu| + |cscale| (|y| + |t|)), and the stored bf16 must be what
 round-to-nearest gives somewhere in [ref - delta, ref + delta] (rn_window).  An element whose mask is <= 0 must be
 exactly 0.
+
+Every case runs a second time on exactly summable operands (gpu_util.check_exact: integer gradients, masks and
+content targets, dyadic weights, Gs, gmu and cscale), where the live outputs must be RN_bf16(ref) bit for bit: the
+window above is wider than one bf16 ulp for many elements at K = 4608, so it cannot see a wrong rounding mode.
 """
 import pytest
 import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
-
-U = 2.0 ** -24
-TILE_H, TILE_W = 16, 8
 
 
 @pytest.fixture(scope='module')
@@ -32,22 +33,6 @@ def G():
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     return g
-
-
-def rn_bf16(x):
-    return x.float().bfloat16().double()
-
-
-def rn_window(got, ref, delta):
-    """True where got is RN_bf16 of some value in [ref - delta, ref + delta] (rounding is monotone)."""
-    return (got >= rn_bf16(ref - delta)) & (got <= rn_bf16(ref + delta))
-
-
-def tiles(H, W, Cout):
-    """CTA tiles of a launch, as launch_pixel_gemm counts them."""
-    bn = 256 if Cout >= 256 else Cout
-    mt = 1 if bn == 256 else 2
-    return -(-H // TILE_H) * -(-W // (TILE_W * mt)) * (Cout // bn)
 
 
 # (name, H, W, channels of A (0: none), Cout, C2, A2 source ('mask', 'other' or None), content target)
@@ -68,21 +53,33 @@ def test_every_cta_walks_three_tiles(G):
     several tiles: fails on a device with more SMs than these shapes were planned for, rather than testing less."""
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     for name, H, W, _, Cout, *_ in CASES:
-        assert tiles(H, W, Cout) // sms >= 3, f'{name}: {tiles(H, W, Cout)} tiles on {sms} SMs'
-    assert tiles(*APRON[:2], APRON[3]) // sms >= 3
+        assert G.tiles(H, W, Cout) // sms >= 3, f'{name}: {G.tiles(H, W, Cout)} tiles on {sms} SMs'
+    assert G.tiles(*APRON[:2], APRON[3]) // sms >= 3
 
 
-def run_case(G, seed, H, W, Cin, Cout, C2, a2_src, content, a2_row0=0, a2_rows=0, row_lo=0, row_hi=1 << 30):
+def run_case(G, seed, H, W, Cin, Cout, C2, a2_src, content, a2_row0=0, a2_rows=0, row_lo=0, row_hi=1 << 30,
+             grid=False):
+    """grid: operands on the dyadic grid (gpu_util.check_exact) and a bit-exact check instead of the RN window."""
     gen = torch.Generator(device='cuda').manual_seed(seed)
     dev = G.DEV
-    y = torch.randn(H, W, Cout, generator=gen, device=dev).bfloat16()          # mask: about half <= 0
+
+    def act(C, lo=-3):        # activations, gradients and the mask: bf16 randn, or integers in [lo, 3]
+        if grid:
+            return G.integers((H, W, C), lo, 3, gen)
+        x = torch.randn(H, W, C, generator=gen, device=dev)
+        return (torch.relu(x) if lo == 0 else x).bfloat16()
+
+    def small(shape, scale):  # weights, Gs, gmu: scaled randn, or dyadic
+        return G.dyadic(shape, gen) if grid else torch.randn(shape, generator=gen, device=dev) * scale
+
+    y = act(Cout)                                                              # mask: about half <= 0
     ref = torch.zeros(H, W, Cout, dtype=torch.float64, device=dev)
     mag = torch.zeros_like(ref)
     kw = {}
     K = 0
     if Cin:
-        go = torch.randn(H, W, Cin, generator=gen, device=dev).bfloat16()
-        w = torch.randn(Cin, Cout, 3, 3, generator=gen, device=dev) * (2.0 / (9 * Cin)) ** 0.5
+        go = act(Cin)
+        w = small((Cin, Cout, 3, 3), (2.0 / (9 * Cin)) ** 0.5)
         g64, w64 = go.double().permute(2, 0, 1)[None], w.bfloat16().double()
         ref += F.conv_transpose2d(g64, w64, padding=1)[0].permute(1, 2, 0)
         mag += F.conv_transpose2d(g64.abs(), w64.abs(), padding=1)[0].permute(1, 2, 0)
@@ -91,9 +88,9 @@ def run_case(G, seed, H, W, Cin, Cout, C2, a2_src, content, a2_row0=0, a2_rows=0
     rows = slice(max(row_lo, 0), min(row_hi, H))
     gmu = torch.zeros(Cout, device=dev)
     if C2:
-        f2 = y if a2_src == 'mask' else torch.randn(H, W, C2, generator=gen, device=dev).bfloat16()
-        gs = (torch.randn(Cout, C2, generator=gen, device=dev) * 0.05).bfloat16()
-        gmu = torch.randn(Cout, generator=gen, device=dev) * 0.1
+        f2 = y if a2_src == 'mask' else act(C2)
+        gs = small((Cout, C2), 0.05).bfloat16()
+        gmu = small((Cout,), 0.1)
         r0, nr = a2_row0, a2_rows or H
         win = f2[r0:r0 + nr]                       # a view: A2 is the mask's rows r0.. when a2_src == 'mask'
         ref[r0:r0 + nr] += (win.double().reshape(-1, C2) @ gs.double().t()).reshape(nr, W, Cout)
@@ -104,8 +101,8 @@ def run_case(G, seed, H, W, Cin, Cout, C2, a2_src, content, a2_row0=0, a2_rows=0
     mag[rows] += gmu.double().abs()
     cs = 0.0
     if content:
-        ct = torch.relu(torch.randn(H, W, Cout, generator=gen, device=dev)).bfloat16()
-        cs = 0.37
+        ct = act(Cout, lo=0)
+        cs = 0.375 if grid else 0.37
         ref[rows] += cs * (y[rows].double() - ct[rows].double())
         mag[rows] += cs * (y[rows].double().abs() + ct[rows].double().abs())
         kw.update(ctarget=ct)
@@ -115,16 +112,26 @@ def run_case(G, seed, H, W, Cin, Cout, C2, a2_src, content, a2_row0=0, a2_rows=0
     dead_bad = live.logical_not() & (got != 0)
     assert not dead_bad.any(), (f'{int(dead_bad.sum())} masked elements are not 0 '
                                 f'(first at {dead_bad.nonzero()[0].tolist()})')
-    delta = 2 * U * (K + 4) * mag
-    bad = live & ~rn_window(got, ref, delta)
+    if grid:
+        G.check_exact(got, ref, mag, live)
+        return None
+    delta = 2 * G.U * (K + 4) * mag
+    bad = live & ~G.rn_window(got, ref, delta)
     assert not bad.any(), (f'{int(bad.sum())} of {int(live.sum())} live elements outside the RN window '
                            f'(first at {bad.nonzero()[0].tolist()}: got {got[tuple(bad.nonzero()[0])].item()}, '
                            f'ref {ref[tuple(bad.nonzero()[0])].item()})')
+    return G.rn_window_ratio(torch.where(live, got, 0), torch.where(live, ref, 0), delta)
 
 
 @pytest.mark.parametrize('name,H,W,Cin,Cout,C2,a2_src,content', CASES, ids=[c[0] for c in CASES])
 def test_dgrad_epilogue_elementwise(G, name, H, W, Cin, Cout, C2, a2_src, content):
-    run_case(G, H * 1000 + W + Cin + C2 + content, H, W, Cin, Cout, C2, a2_src, content)
+    r = run_case(G, H * 1000 + W + Cin + C2 + content, H, W, Cin, Cout, C2, a2_src, content)
+    print(f'RATIO dgrad_epilogue {name} {r:.3g}')
+
+
+@pytest.mark.parametrize('name,H,W,Cin,Cout,C2,a2_src,content', CASES, ids=[c[0] for c in CASES])
+def test_dgrad_epilogue_exact_on_dyadic_grid(G, name, H, W, Cin, Cout, C2, a2_src, content):
+    run_case(G, H * 1000 + W + Cin + C2 + content + 1, H, W, Cin, Cout, C2, a2_src, content, grid=True)
 
 
 # a band computing its aprons: the output covers the whole local image, A2 (a view of the mask) only the own rows
@@ -135,4 +142,10 @@ def test_dgrad_epilogue_apron_window_streams_the_mask(G):
     """A2 is the mask's rows [r0, r0 + rows), the launch computes all H rows: outside the window the kernel must take
     the mask from the mask tensor (the A2 box is zero-filled there), inside it adds gmu and the tap gradient."""
     H, W, Cin, C, r0, nr = APRON
-    run_case(G, 11, H, W, Cin, C, C, 'mask', False, a2_row0=r0, a2_rows=nr, row_lo=r0, row_hi=r0 + nr)
+    r = run_case(G, 11, H, W, Cin, C, C, 'mask', False, a2_row0=r0, a2_rows=nr, row_lo=r0, row_hi=r0 + nr)
+    print(f'RATIO dgrad_epilogue apron {r:.3g}')
+
+
+def test_dgrad_epilogue_apron_window_exact_on_dyadic_grid(G):
+    H, W, Cin, C, r0, nr = APRON
+    run_case(G, 12, H, W, Cin, C, C, 'mask', False, a2_row0=r0, a2_rows=nr, row_lo=r0, row_hi=r0 + nr, grid=True)

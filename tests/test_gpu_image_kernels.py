@@ -63,34 +63,6 @@ def nchw(x_hwc):
 
 
 # ------------------------------------------------------------------------------------------------ reference helpers
-def rn_bf16(x):
-    """Round-to-nearest-even to bf16, as a float64 tensor.  Through fp32: both steps are monotone, which is all the
-    window test below needs."""
-    return x.float().bfloat16().double()
-
-
-def rn_window(got, ref, delta, relu=False):
-    """True where `got` is what RN_bf16 gives somewhere in [ref - delta, ref + delta]: the kernel's fp32 value lies in
-    that interval, and rounding is monotone, so RN of it lies between RN(ref - delta) and RN(ref + delta).  relu:
-    the kernel rounds max(acc, 0), and RN commutes with max(., 0)."""
-    lo, hi = rn_bf16(ref - delta), rn_bf16(ref + delta)
-    if relu:
-        lo, hi = lo.clamp_min(0), hi.clamp_min(0)
-    return (got >= lo) & (got <= hi)
-
-
-def rn_window_ratio(got, ref, delta, relu=False):
-    """Largest |ref - b| / delta over the elements where got != RN(ref), b the rounding boundary between the two
-    (<= 1 when the window test passes); 0 if every element is RN(ref)."""
-    rn = rn_bf16(ref)
-    off = got != rn
-    if relu:
-        off &= (got > 0) & (rn > 0)
-    if not off.any():
-        return 0.0
-    return ((ref - (got + rn) / 2).abs() / delta)[off].max().item()
-
-
 def conv0_fwd_ref(img, w0, b0):
     """conv0 pre-activation conv(pad(normalise(x)), bf16(w0)) + b in float64 and its magnitude
     A = conv(|v|, |bf16(w0)|) + |b|; img [1,3,H,W] fp32, result [1,64,H,W]."""
@@ -265,10 +237,10 @@ def test_conv0_forward_elementwise(G, conv0_weights, H, W):
     pre, A = conv0_fwd_ref(img, w0, b0)
     got = nchw(out).double()
     delta = 2.0 ** -15 * A
-    ok = rn_window(got, pre, delta, relu=True)
+    ok = G.rn_window(got, pre, delta, relu=True)
     bad = int((~ok).sum())
     assert bad == 0, f'{bad} of {ok.numel()} elements outside the RN window (first at {(~ok).nonzero()[0].tolist()})'
-    print(f'RATIO conv0_fwd {H}x{W} {rn_window_ratio(got, pre, delta, relu=True):.3g}')
+    print(f'RATIO conv0_fwd {H}x{W} {G.rn_window_ratio(got, pre, delta, relu=True):.3g}')
 
 
 # ------------------------------------------------------------------------------------------------ conv0 backward
@@ -437,19 +409,21 @@ def test_pool_backward_elementwise(G, C, H, W, pooling):
         assert not bad.any(), f'{int(bad.sum())} elements differ (first at {bad.nonzero()[0].tolist()})'
         return
     delta = 2.0 ** -21 * ref.abs()
-    ok = rn_window(got, ref, delta)
+    ok = G.rn_window(got, ref, delta)
     assert ok.all(), f'{int((~ok).sum())} elements outside the RN window (first at {(~ok).nonzero()[0].tolist()})'
-    print(f'RATIO pool_bwd_l2 {C},{H},{W} {rn_window_ratio(got.abs(), ref.abs(), delta):.3g}')
+    print(f'RATIO pool_bwd_l2 {C},{H},{W} {G.rn_window_ratio(got.abs(), ref.abs(), delta):.3g}')
 
 
 # ------------------------------------------------------------------------------------------------ fused pool forward
 @pytest.mark.parametrize('H,W,Cin,Cout', [(362, 512, 64, 64), (181, 256, 128, 128), (91, 64, 256, 256),
-                                          (45, 33, 512, 512)])
+                                          (45, 33, 512, 512), (32, 24, 64, 64), (37, 21, 64, 128), (18, 50, 128, 256),
+                                          (6, 6, 512, 512)])
 @pytest.mark.parametrize('pooling', ['max', 'average', 'l2'])
 def test_fused_pool_forward_elementwise(G, H, W, Cin, Cout, pooling):
     """The pool of the conv output as stored (bf16), floor mode.  Max: bit-exact.  Average: bit-exact against the
     epilogue's fp32 arithmetic, ((a + b) + c) + d, * 0.25, * 2 (exact), RN to bf16 (the build uses no fast-math).
-    L2: sqrtf of a sum of four exact squares (3 u / 2 + u / 2), * 0.78f (2 u): RN_bf16(ref) within 2^-21 |ref|."""
+    L2: sqrtf of a sum of four exact squares (3 u / 2 + u / 2), * 0.78f (2 u): RN_bf16(ref) within 2^-21 |ref|.
+    The stored conv output itself is checked element by element in test_gpu_pixel_gemm.py, on the same launches."""
     code = {'max': 0, 'average': 1, 'l2': 2}[pooling]
     gen = _gen(H * W + Cout)
     x = torch.randn(H, W, Cin, generator=gen, device=G.DEV).bfloat16()
@@ -471,9 +445,9 @@ def test_fused_pool_forward_elementwise(G, H, W, Cin, Cout, pooling):
     else:
         r64 = (a.double() ** 2 + bb.double() ** 2 + c.double() ** 2 + d.double() ** 2).sqrt() * 0.78
         delta = 2.0 ** -21 * r64
-        ok = rn_window(pooled.double(), r64, delta)
+        ok = G.rn_window(pooled.double(), r64, delta)
         assert ok.all(), f'{int((~ok).sum())} pooled elements outside the RN window'
-        print(f'RATIO pool_fwd_l2 {H}x{W}x{Cout} {rn_window_ratio(pooled.double(), r64, delta):.3g}')
+        print(f'RATIO pool_fwd_l2 {H}x{W}x{Cout} {G.rn_window_ratio(pooled.double(), r64, delta):.3g}')
         return
     bad = ~(pooled == ref)
     assert not bad.any(), f'{int(bad.sum())} pooled elements differ (first at {bad.nonzero()[0].tolist()})'
