@@ -167,6 +167,24 @@ STB_API int stb_set_loss_ring(stb_ctx* ctx, float* host_ring, int slots);
 STB_API int stb_resize(const float* in, int C, int H, int W, float* out, int Ho, int Wo, int mode, int post,
                        void* stream);
 
+/* ------------------------------------------------------------------ source images (ST:417, 437)
+ * out[1,3,rows,Wo] fp32 planar = rows [row0, row0 + rows) of TF.to_tensor(Image.resize((Wo, Ho), Image.BICUBIC)) of the
+ * 8-bit RGB image src[Hs][Ws][3] (device, interleaved), bit for bit: Pillow's two fixed-point passes (horizontal first,
+ * its result stored as uint8; a pass whose axis keeps its size is skipped) and value = u8 * (1.0f / 255.0f), which is
+ * what torch computes for `.to(float32).div_(255)` on the device.  A row window costs the source rows it needs only.
+ *   kx / ky : device int32 [Wo][ksize_x] / [Ho][ksize_y], the weights of every output sample with 22 fractional bits
+ *   bx / by : device int32 [Wo][2] / [Ho][2], (first input sample, number of taps) of every output sample
+ *             an output sample is clip8((2^21 + sum_j in[first + j] * k[j]) >> 22); the tables are Pillow's, built by
+ *             the caller in double (style_transfer.resample_coeffs); those of an axis that keeps its size are ignored
+ *   tmp     : caller-owned scratch of stb_resample_tmp_bytes(...) bytes (0 when Ws == Wo: may be NULL then)
+ * The bounds are clamped to the image, so tables of other sizes give wrong pixels but no access outside src / tmp.
+ * STB_ERR_INVALID, with nothing launched, for a null src / out / needed table, a size < 1, a window that is empty or
+ * not inside [0, Ho), or a scratch that is missing or too small. */
+STB_API int stb_resample_tmp_bytes(int Hs, int Ws, int Ho, int Wo, int row0, int rows, size_t* bytes);
+STB_API int stb_resample_rgb8(const uint8_t* src, int Hs, int Ws, int Ho, int Wo, int row0, int rows,
+                              const int32_t* kx, const int32_t* bx, int ksize_x, const int32_t* ky, const int32_t* by,
+                              int ksize_y, void* tmp, size_t tmp_bytes, float* out, void* stream);
+
 /* ------------------------------------------------------------------ image snapshot (get_image, periodic saves)
  * value: planar fp32 [3][H][W] (the EMA's storage); out: interleaved [H][W][3], written in one pass on `stream`.
  *   kind 0: uint8  = trunc(clamp(value / denom, 0, 1) * 255)       (to_pil_image: mul(255).byte())

@@ -60,6 +60,8 @@ def _declare(lib):
         'stb_set_loss_ring': [vp, vp, i],
         'stb_resize': [vp, i, i, i, vp, i, i, i, i, vp],
         'stb_snapshot': [vp, i, i, C.c_double, i, vp, vp],
+        'stb_resample_tmp_bytes': [i, i, i, i, i, i, C.POINTER(sz)],
+        'stb_resample_rgb8': [vp, i, i, i, i, i, i, vp, vp, i, vp, vp, i, vp, sz, vp, vp],
         'stb_comm_create': [vp, i, i, i, i, vp, pp],
         'stb_comm_connect_ipc': [vp, vp],
         'stb_comm_connect_local': [vp, pp],
@@ -121,7 +123,8 @@ EXPORTS = [
     'stb_set_layers', 'stb_content_features_ex', 'stb_set_targets_ex', 'stb_loss_terms',
     'stb_lbfgs_state_bytes', 'stb_lbfgs_reset', 'stb_iterate_lbfgs',
     'stb_set_band', 'stb_stats_block', 'stb_iterate_fwd', 'stb_iterate_bwd', 'stb_adam_update',
-    'stb_set_loss_ring', 'stb_resize', 'stb_snapshot', 'stb_comm_create', 'stb_comm_connect_ipc', 'stb_comm_connect_local', 'stb_comm_disconnect', 'stb_comm_alloc_workspace',
+    'stb_set_loss_ring', 'stb_resize', 'stb_snapshot', 'stb_resample_tmp_bytes', 'stb_resample_rgb8',
+    'stb_comm_create', 'stb_comm_connect_ipc', 'stb_comm_connect_local', 'stb_comm_disconnect', 'stb_comm_alloc_workspace',
     'stb_comm_connect_ws_ipc', 'stb_comm_connect_ws_local', 'stb_comm_release_workspace',
     'stb_comm_set_geometry', 'stb_comm_reset',
     'stb_iterate_banded', 'stb_iterate_lbfgs_banded', 'stb_graph_status', 'stb_launch_count', 'stb_profile_enable', 'stb_profile_read', 'stb_debug_activation', 'stb_debug_w2_trace',

@@ -1229,6 +1229,19 @@ int stb_snapshot(const float* value, int H, int W, double denom, int kind, void*
   return launch_snapshot(value, H, W, denom, kind, out, static_cast<cudaStream_t>(stream));
 }
 
+// Source images (SURVEY.md 8f row 1, ST:417, 437): the content and style images are uploaded once as uint8 and every
+// scale's tensors come from them by Pillow's bicubic resize restated on the device (csrc/resample.cu).
+int stb_resample_tmp_bytes(int Hs, int Ws, int Ho, int Wo, int row0, int rows, size_t* bytes) {
+  return resample_tmp_bytes(Hs, Ws, Ho, Wo, row0, rows, bytes);
+}
+
+int stb_resample_rgb8(const uint8_t* src, int Hs, int Ws, int Ho, int Wo, int row0, int rows, const int32_t* kx,
+                      const int32_t* bx, int ksize_x, const int32_t* ky, const int32_t* by, int ksize_y, void* tmp,
+                      size_t tmp_bytes, float* out, void* stream) {
+  return launch_resample_rgb8(src, Hs, Ws, Ho, Wo, row0, rows, kx, bx, ksize_x, ky, by, ksize_y, tmp, tmp_bytes, out,
+                              static_cast<cudaStream_t>(stream));
+}
+
 int stb_iterate(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, float* ema, int64_t step, float lr,
                 float beta1, float beta2, float adam_eps, float ema_decay, float* loss_out_host8, void* stream) {
   return stb_iterate_ex(ctx, img, exp_avg, exp_avg_sq, ema, step, lr, beta1, beta2, adam_eps, ema_decay, 1, nullptr,
@@ -1324,6 +1337,7 @@ int stb_comm_create(stb_ctx* ctx, int rank, int world, int max_h_local, int max_
   // every kernel of an iteration must be loaded before a peer-wait kernel can be resident (see comm_preload)
   STB_TRY(comm_preload()); STB_TRY(preload_conv_kernels()); STB_TRY(preload_gram_kernels());
   STB_TRY(preload_w2_kernels()); STB_TRY(preload_conv0_kernels()); STB_TRY(preload_image_kernels());
+  STB_TRY(preload_resample_kernels());
   cudaFuncAttributes fa;
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(reduce_partials_kernel)));
   STB_CUDA_CHECK(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(content_seed_kernel)));

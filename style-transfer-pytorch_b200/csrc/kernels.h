@@ -99,6 +99,15 @@ int launch_resize(const float* in, int C, int H, int W, float* out, int Ho, int 
 // fp32 [3][H][W] / denom, clamped to [0,1], quantised to interleaved [H][W][3]: kind 0 uint8, 1 uint16 (stb_snapshot)
 int launch_snapshot(const float* value, int H, int W, double denom, int kind, void* out, cudaStream_t s);
 
+// ---------------------------------------------------------------- source images (resample.cu)
+// out fp32 planar [3][rows][Wo] = rows [row0, row0 + rows) of to_tensor(Image.resize((Wo, Ho), BICUBIC)) of the uint8 RGB
+// image src[Hs][Ws][3] (stb_resample_rgb8); tmp: resample_tmp_bytes(...) bytes for the horizontal pass's result
+int resample_tmp_bytes(int Hs, int Ws, int Ho, int Wo, int row0, int rows, size_t* bytes);
+int launch_resample_rgb8(const uint8_t* src, int Hs, int Ws, int Ho, int Wo, int row0, int rows, const int32_t* kx,
+                         const int32_t* bx, int ksize_x, const int32_t* ky, const int32_t* by, int ksize_y, void* tmp,
+                         size_t tmp_bytes, float* out, cudaStream_t s);
+int preload_resample_kernels();
+
 // ---------------------------------------------------------------- L-BFGS step on the device (lbfgs.cu)
 // torch.optim.LBFGS.step (lr 1, max_iter 1, history STB_LBFGS_HISTORY, no line search) + EMA on n-float vectors; the
 // state is one caller-owned block of lbfgs_state_bytes(n) bytes (256-byte aligned), reset by launch_lbfgs_reset.

@@ -4,8 +4,9 @@ Public surface mirrors /root/reference/style_transfer/style_transfer.py ("ST"): 
 (ST:310), attributes (ST:311-324), `get_image_tensor` / `get_image` (ST:335-347), `stylize(...)` with the same
 keyword-only signature, defaults and annotations (ST:349-363; the CLI scrapes them, cli.py:150-153), `STIterate`
 (ST:298-306) and the synchronous per-iteration callback (ST:487-493).  Host-side work that is per *scale*, not per
-iteration (PIL resizes, init modes, bicubic warm start of the Adam moments) stays in PyTorch; everything inside
-the iteration loop (ST:472-486) runs in the native library.  There is no CPU or autograd fallback.
+iteration (the random init modes, the per-scale bookkeeping) stays in PyTorch; everything inside the iteration loop
+(ST:472-486) runs in the native library, and so do the per-scale resizes of the source images (SourceImage) and the
+warm start.  There is no CPU or autograd fallback.
 """
 from __future__ import annotations
 
@@ -90,6 +91,80 @@ def _pil_to_tensor(img, device=None):
     if device is not None:
         t = t.to(device, non_blocking=True)
     return t.permute(2, 0, 1).to(torch.float32).div_(255).unsqueeze(0).contiguous()
+
+
+def resample_coeffs(in_size, out_size):
+    """Fixed-point tables of one axis of `Image.resize(..., Image.BICUBIC)` on 8-bit pixels, from `in_size` to `out_size`
+    samples: (k int32 [out_size, ksize], bounds int32 [out_size, 2]).  Output sample x is
+    clip8((2^21 + sum_j source[first + j] * k[x, j]) >> 22) over j < count, with (first, count) = bounds[x]; taps
+    beyond count are zero.  Pillow forms the weights in double: the Keys kernel (a = -0.5) stretched by
+    max(in / out, 1), divided by their sum accumulated in tap order, rounded half away from zero to 22 fractional
+    bits.  The loop below runs over the taps so that every sum is taken in that order (np.sum adds pairwise)."""
+    scale = in_size / out_size
+    filterscale = max(scale, 1.0)
+    support = 2.0 * filterscale
+    ksize = 2 * int(np.ceil(support)) + 1
+    center = (np.arange(out_size, dtype=np.float64) + 0.5) * scale
+    first = np.maximum((center - support + 0.5).astype(np.int64), 0)       # astype truncates, as C's (int)
+    count = np.minimum((center + support + 0.5).astype(np.int64), in_size) - first
+    inv = 1.0 / filterscale
+    w = np.zeros((out_size, ksize), dtype=np.float64)
+    total = np.zeros(out_size, dtype=np.float64)
+    for j in range(ksize):
+        t = np.abs((j + first - center + 0.5) * inv)
+        near = ((-0.5 + 2.0) * t - (-0.5 + 3.0)) * t * t + 1
+        far = (((t - 5) * t + 8) * t - 4) * -0.5
+        w[:, j] = np.where(j < count, np.where(t < 1.0, near, np.where(t < 2.0, far, 0.0)), 0.0)
+        total += w[:, j]
+    total[total == 0.0] = 1.0
+    w /= total[:, None]
+    k = (w * float(1 << 22) + np.where(w < 0, -0.5, 0.5)).astype(np.int32)
+    return k, np.stack([first, count], axis=1).astype(np.int32)
+
+
+class SourceImage:
+    """One content or style image of a stylize() call, resampled to every scale on the device.
+
+    An RGB image is uploaded once, as interleaved uint8 [Hs][Ws][3]; resized() then produces what
+    `_pil_to_tensor(img.resize((w, h), Image.BICUBIC), device)` produces, bit for bit, by stb_resample_rgb8.  Pillow
+    resamples every other mode (RGBA, P, I;16, F, ...) by other rules, so such an image keeps that expression: it is
+    resized in its own mode on the host and converted afterwards."""
+
+    def __init__(self, img, device):
+        self.img, self.device = img, device
+        self.data = None
+        if img.mode == 'RGB':
+            self.data = torch.from_numpy(np.array(img, dtype=np.uint8)).to(device, non_blocking=True)
+
+    def resized(self, w, h, row0=0, rows=None):
+        """Rows [row0, row0 + rows) (default: all) of the image at w x h: [1,3,rows,w] fp32 in [0,1] on the device."""
+        rows = h - row0 if rows is None else rows
+        if self.data is None:
+            full = _pil_to_tensor(self.img.resize((w, h), Image.BICUBIC), self.device)
+            return full[:, :, row0:row0 + rows].contiguous()
+        hs, ws, _ = self.data.shape
+        lib = _lib.load()
+        need = ctypes.c_size_t()
+        _lib.check(lib.stb_resample_tmp_bytes(hs, ws, h, w, row0, rows, ctypes.byref(need)))   # validates the window
+        # an axis that keeps its size is not filtered (Pillow skips that pass) and has no tables
+        axes = [resample_coeffs(n_in, n_out) if n_in != n_out else None for n_in, n_out in ((ws, w), (hs, h))]
+        flat = [t.ravel() for axis in axes if axis is not None for t in axis]
+        with torch.cuda.device(self.device):
+            tab = torch.from_numpy(np.concatenate(flat)).to(self.device) if flat else None   # one upload for all four
+            tmp = torch.empty(need.value, dtype=torch.uint8, device=self.device)
+            out = torch.empty(1, 3, rows, w, dtype=torch.float32, device=self.device)
+            args, off = [], 0
+            for axis in axes:
+                if axis is None:
+                    args += [None, None, 0]
+                    continue
+                k, bounds = axis
+                args += [ctypes.c_void_p(tab.data_ptr() + 4 * off), ctypes.c_void_p(tab.data_ptr() + 4 * (off + k.size)),
+                         k.shape[1]]
+                off += k.size + bounds.size
+            _lib.check(lib.stb_resample_rgb8(_lib.ptr(self.data), hs, ws, h, w, row0, rows, *args,
+                                             _lib.ptr(tmp), need.value, _lib.ptr(out), _lib.cur_stream()))
+        return out
 
 
 def load_vgg19_conv_weights():
@@ -622,8 +697,6 @@ class StyleTransfer:
 
     # ------------------------------------------------------------------ helpers
     def _initial_image(self, init, content_image, style_images, style_weights, cw, ch):
-        if init == 'content':
-            return _pil_to_tensor(content_image.resize((cw, ch), Image.BICUBIC))
         if init == 'gray':
             return torch.rand([1, 3, ch, cw]) / 255 + 0.5
         if init == 'uniform':
@@ -762,16 +835,21 @@ class StyleTransfer:
         m.comm_set_geometry(w, band, up, down, self._halo_now)
 
     def _style_stats(self, simg, sh, sw):
-        """(means, second raw moments) of one style image (ST:440-443).  Under torch.distributed a large style image
+        """(means, second raw moments) of one style image (ST:440-443) at sw x sh: a [1,3,sh,sw] tensor, or a
+        SourceImage, of which only the rows that are needed are resampled.  Under torch.distributed a large style image
         is tiled like the iterate: every rank runs its band, the raw sums are all-reduced once (per scale, not per
         iteration), and the global pixel counts normalise them."""
         m = self.model
         band = D.make_band(sh, self._rank, self._world) if self._dist else None
         if band is None:
             m.set_band(False)
-            return m.style_stats(simg)
+            return m.style_stats(simg.resized(sw, sh) if isinstance(simg, SourceImage) else simg)
         m.set_band(True, sh, band.own0, band.own_rows)
-        means, srms = m.style_stats(D.local_slice(simg, band))      # RAW sums over this band's own rows
+        if isinstance(simg, SourceImage):
+            local = simg.resized(sw, sh, band.loc_begin, band.h_local)
+        else:
+            local = D.local_slice(simg, band)
+        means, srms = m.style_stats(local)      # RAW sums over this band's own rows
         m.set_band(False)
         if not means:
             return means, srms
@@ -969,10 +1047,11 @@ class StyleTransfer:
 
         scales = gen_scales(min_scale, end_scale)
         cw, ch = size_to_fit(content_image.size, scales[0], scale_up=True)
-        first_content = None
-        if init == 'content':  # the initial iterate IS the first scale's content tensor: convert/upload it once
-            first_content = _pil_to_tensor(content_image.resize((cw, ch), Image.BICUBIC), dev)
-            self.image = first_content.clone()
+        # the full-size images go to the device once; every scale resamples them there
+        content_src = SourceImage(content_image, dev)
+        style_srcs = [SourceImage(simg, dev) for simg in style_images]
+        if init == 'content':
+            self.image = content_src.resized(cw, ch)
         else:
             self.image = self._initial_image(init, content_image, style_images, style_weights, cw, ch).to(dev)
             if self._dist:  # random inits are drawn per process: every rank continues from rank 0's draw
@@ -987,17 +1066,13 @@ class StyleTransfer:
                 torch.cuda.empty_cache()
 
                 cw, ch = size_to_fit(content_image.size, scale, scale_up=True)
-                if scale == scales[0] and first_content is not None:
-                    content, first_content = first_content, None
-                else:
-                    content = _pil_to_tensor(content_image.resize((cw, ch), Image.BICUBIC), dev)
                 styles = []
-                for simg in style_images:
+                for simg, src in zip(style_images, style_srcs):
                     if style_size is None:
                         sw, sh = size_to_fit(simg.size, round(scale * style_scale_fac))
                     else:
                         sw, sh = size_to_fit(simg.size, style_size)
-                    styles.append((sw, sh, _pil_to_tensor(simg.resize((sw, sh), Image.BICUBIC), dev)))
+                    styles.append((sw, sh, src))
                 # multi-GPU: tile this scale into horizontal bands (None: too small, every rank runs the whole image).
                 # L-BFGS is tiled only with the exchanges inside the library ('peer'): its step needs 22 cross-rank
                 # reductions per iteration, which run as kernels in the iteration's graph.  Under host-driven NCCL
@@ -1030,10 +1105,11 @@ class StyleTransfer:
                 self.model.ensure_workspace([(h_loc, cw)] + style_sizes)
 
                 self.image = self.model.resize(self.image, (ch, cw), 'bicubic', 'clamp')          # ST:420
-                if band is not None:
-                    full_image = self.image
-                    self.image = D.local_slice(full_image, band)
-                    content = D.local_slice(content, band)
+                if band is not None:   # the band's rows only: the full-height content tensor is never formed
+                    self.image = D.local_slice(self.image, band)
+                    content = content_src.resized(cw, ch, band.loc_begin, band.h_local)
+                else:
+                    content = content_src.resized(cw, ch)
                 self.average = EMA(self.image, avg_decay)
                 self._band = band   # from here on the average holds the band's rows only
 
