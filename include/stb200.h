@@ -138,20 +138,16 @@ STB_API int stb_iterate_lbfgs(stb_ctx* ctx, float* img, float* ema, void* state,
  * A context may work on a horizontal band (plus halo aprons) of a taller image: H passed to the other calls is the
  * LOCAL height, rows [own_row0, own_row0+own_rows) (multiples of 16) are the band's own rows, H_global the full
  * height.  Only own rows enter the statistics, losses and tap gradients.  An iteration of a band is one call of
- * stb_iterate_banded (or stb_iterate_lbfgs_banded), with the exchanges between the ranks inside it (below).  Where the
- * ranks cannot map each other's memory, the host drives the same iteration in phases instead:
- *   stb_iterate_fwd  -> all-reduce(sum) of the stats block over the ranks (one NCCL call, ~2.4 MB)
- *   stb_iterate_bwd  -> grad_out = d loss / d (local image) incl. contributions to the halo rows
- *   [exchange + add the halo rows of grad_out with the neighbouring bands]
- *   stb_adam_update  on the own rows, then refresh the halo rows of the image from the neighbours.
+ * stb_iterate_banded (or stb_iterate_lbfgs_banded), with the exchanges between the ranks inside it (below).
+ * stb_iterate_fwd and stb_iterate_bwd are the closure (no update) split in two: the forward and statistics, then the
+ * losses and the backward into grad_out = d loss / d (local image), halo rows included.  Between the two halves the
+ * statistics block (Gram sums, channel sums, content SSE, TV sum), whose device address stb_stats_block returns, can be
+ * read and overwritten, e.g. with statistics summed over the bands of all ranks.
  * With a band set, stb_style_stats returns RAW sums over the own rows (all-reduce, then divide by the global count). */
 STB_API int stb_set_band(stb_ctx* ctx, int enabled, int H_global, int own_row0, int own_rows);
 STB_API int stb_stats_block(stb_ctx* ctx, int H, int W, float** dev_ptr, size_t* n_floats);
 STB_API int stb_iterate_fwd(stb_ctx* ctx, const float* img, void* stream);
 STB_API int stb_iterate_bwd(stb_ctx* ctx, float* img, float* grad_out, float* loss_out_host8, void* stream);
-STB_API int stb_adam_update(float* img, const float* grad, float* exp_avg, float* exp_avg_sq, float* ema, int H, int W,
-                            int row0, int rows, int64_t step, float lr, float beta1, float beta2, float adam_eps,
-                            float ema_decay, void* stream);
 
 /* ------------------------------------------------------------------ sync-free loss read-back (ST:487-493)
  * host_ring: PINNED host memory, slots x 16 floats (NULL switches it off).  Each updating iteration stores its loss-term

@@ -56,7 +56,6 @@ def _declare(lib):
         'stb_stats_block': [vp, i, i, pp, C.POINTER(sz)],
         'stb_iterate_fwd': [vp, vp, vp],
         'stb_iterate_bwd': [vp, vp, vp, vp, vp],
-        'stb_adam_update': [vp, vp, vp, vp, vp, i, i, i, i, i64, f, f, f, f, f, vp],
         'stb_set_loss_ring': [vp, vp, i],
         'stb_resize': [vp, i, i, i, vp, i, i, i, i, vp],
         'stb_snapshot': [vp, i, i, C.c_double, i, vp, vp],
@@ -122,7 +121,7 @@ EXPORTS = [
     'stb_style_stats', 'stb_content_features', 'stb_set_targets', 'stb_iterate', 'stb_iterate_ex',
     'stb_set_layers', 'stb_content_features_ex', 'stb_set_targets_ex', 'stb_loss_terms',
     'stb_lbfgs_state_bytes', 'stb_lbfgs_reset', 'stb_iterate_lbfgs',
-    'stb_set_band', 'stb_stats_block', 'stb_iterate_fwd', 'stb_iterate_bwd', 'stb_adam_update',
+    'stb_set_band', 'stb_stats_block', 'stb_iterate_fwd', 'stb_iterate_bwd',
     'stb_set_loss_ring', 'stb_resize', 'stb_snapshot', 'stb_resample_tmp_bytes', 'stb_resample_rgb8',
     'stb_comm_create', 'stb_comm_connect_ipc', 'stb_comm_connect_local', 'stb_comm_disconnect', 'stb_comm_alloc_workspace',
     'stb_comm_connect_ws_ipc', 'stb_comm_connect_ws_local', 'stb_comm_release_workspace',

@@ -9,7 +9,6 @@
 #include <cstring>
 #include <string>
 
-#include "comm.cuh"
 #include "kernels.h"
 #include "ptx.cuh"
 
@@ -420,18 +419,6 @@ __global__ void content_seed_kernel(const bf16* __restrict__ y, const bf16* __re
     const float yv = __bfloat162float(y[i]);
     const float v = (row >= row_lo && row < row_hi) ? cscale * (yv - __bfloat162float(t[i])) : 0.f;
     g[i] = __float2bfloat16(yv > 0.f ? v : 0.f);
-  }
-}
-
-__global__ void adam_rows_kernel(float* __restrict__ img, const float* __restrict__ grad, float* __restrict__ exp_avg,
-                                 float* __restrict__ exp_avg_sq, float* __restrict__ ema, int H, int W, int row0,
-                                 int rows, AdamScalars ac) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 3 * rows * W; i += gridDim.x * blockDim.x) {
-    const long idx = row_pos<1>(i, rows, W, H, row0).off;
-    const float g = grad[idx];
-    float m = exp_avg[idx], v = exp_avg_sq[idx], p = img[idx], e = ema[idx];
-    adam_element(ac, g, m, v, p, e);
-    exp_avg[idx] = m; exp_avg_sq[idx] = v; img[idx] = p; ema[idx] = e;
   }
 }
 
@@ -1015,7 +1002,7 @@ enum Update { UPDATE_NONE, UPDATE_ADAM_FUSED, UPDATE_ADAM_SEAM, UPDATE_LBFGS, UP
 struct Variant {
   const char* name;   // the entry point, for the error texts
   GraphSlotId slot;
-  bool fwd, bwd;      // records the forward / the backward half (the host-driven phases of a band record one each)
+  bool fwd, bwd;      // records the forward / the backward half (stb_iterate_fwd / stb_iterate_bwd record one each)
   bool banded;
   StepKernel step;
   Update update;      // ADAM_FUSED: in the epilogue of conv0's dgrad; ADAM_SEAM / LBFGS_BANDED: after the seam exchange
@@ -1161,9 +1148,9 @@ int stb_iterate_ex(stb_ctx* ctx, float* img, float* exp_avg, float* exp_avg_sq, 
   return iterate(ctx, apply_update ? kIterate : kClosure, a, apply_update && grad_out == nullptr, stream);
 }
 
-// ---- spatial tiling across GPUs (SURVEY.md section 8e).  A band's iteration is stb_iterate_banded; without peer
-// memory the host drives its phases: stb_iterate_fwd -> all-reduce(stats block) -> stb_iterate_bwd -> seam exchange
-// of grad -> stb_adam_update
+// ---- spatial tiling across GPUs (SURVEY.md section 8e).  A band's iteration is stb_iterate_banded; stb_iterate_fwd /
+// stb_iterate_bwd are the closure split in two, with the statistics block (stb_stats_block) readable and writable
+// between the halves
 int stb_set_band(stb_ctx* ctx, int enabled, int H_global, int own_row0, int own_rows) {
   STB_CHECK(ctx != nullptr, STB_ERR_INVALID, "null ctx");
   if (enabled) {
@@ -1197,23 +1184,6 @@ int stb_iterate_bwd(stb_ctx* ctx, float* img, float* grad_out, float* loss_out_h
   a.grad_out = grad_out;
   a.loss_out_host8 = loss_out_host8;
   return iterate(ctx, kBwd, a, true, stream);
-}
-
-// Adam + clamp + EMA on rows [row0, row0+rows) of [3][H][W] fp32 tensors (the band's own rows, host-driven phases)
-int stb_adam_update(float* img, const float* grad, float* exp_avg, float* exp_avg_sq, float* ema, int H, int W,
-                    int row0, int rows, int64_t step, float lr, float beta1, float beta2, float adam_eps,
-                    float ema_decay, void* stream) {
-  STB_CHECK(img && grad && exp_avg && exp_avg_sq && ema, STB_ERR_INVALID, "null argument");
-  STB_CHECK(row0 >= 0 && rows > 0 && row0 + rows <= H && step >= 1, STB_ERR_INVALID, "bad row range / step");
-  STB_CHECK(3l * rows * W < (1l << 31), STB_ERR_INVALID, "band of %d x %d pixels is too large", rows, W);
-  const AdamScalars as = make_adam_scalars(step, lr, beta1, beta2, adam_eps, ema_decay);
-  const long n = 3l * rows * W;
-  long blocks = (n + 255) / 256;
-  if (blocks > 16l * num_sms()) blocks = 16l * num_sms();
-  adam_rows_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(img, grad, exp_avg, exp_avg_sq, ema, H,
-                                                                                  W, row0, rows, as);
-  STB_CUDA_CHECK(cudaGetLastError());
-  return STB_OK;
 }
 
 // Per-scale warm start on the device (SURVEY.md 8f row 1): F.interpolate(in[1,C,H,W], (Ho,Wo), mode, align_corners=

@@ -1,8 +1,8 @@
 // Device-side primitives of the peer-memory exchange (comm.cu, and the cross-rank reductions of the banded L-BFGS step
 // in lbfgs.cu): system-scope release / acquire of the iteration stamps, the bounded wait for a peer's stamp, and loads
 // of peer data that bypass a possibly stale L1 line.  Also the one home of what every banded row kernel (comm.cu,
-// lbfgs.cu, api.cu) must agree on bit for bit: the row vector, the walk over a band's rows, the seam sum of the image
-// gradient and the outbox layout.
+// lbfgs.cu) must agree on bit for bit: the row vector, the walk over a band's rows, the seam sum of the image gradient
+// and the outbox layout.
 #pragma once
 
 #include <type_traits>

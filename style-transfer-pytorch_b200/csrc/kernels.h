@@ -48,8 +48,8 @@ int pack_weights_bwd(const float* w, bf16* out, int Cout, int Cin, cudaStream_t 
 struct AdamScalars {  // torch/optim/adam.py:413-546 scalars, evaluated on the host in double like torch does
   float one_minus_b1, b2, one_minus_b2, step_size, inv_sqrt_bc2, eps, ema_decay, one_minus_decay;
 };
-// the scalars of Adam step `step` (1-based): on the host for stb_adam_update, on the device by adam_scalars_kernel
-// (each side with its own pow / sqrt)
+// the scalars of Adam step `step` (1-based): on the device by adam_scalars_kernel, on the host by the test library's
+// stb_test_conv0_bwd_adam (each side with its own pow / sqrt)
 __host__ __device__ inline AdamScalars make_adam_scalars(int64_t step, float lr, float beta1, float beta2,
                                                          float adam_eps, float ema_decay) {
   AdamScalars as{};
@@ -62,7 +62,7 @@ __host__ __device__ inline AdamScalars make_adam_scalars(int64_t step, float lr,
   return as;
 }
 // Adam + clamp to [0, 1] + EMA of one element: moments m, v, image p, EMA e; g is the gradient.  Every Adam update
-// (conv0's fused epilogues, the band seam, stb_adam_update's rows) runs this one copy, so they all round alike.
+// (conv0's fused epilogues, the band seam) runs this one copy, so they all round alike.
 __device__ __forceinline__ void adam_element(const AdamScalars& ac, float g, float& m, float& v, float& p, float& e) {
   m = m + (g - m) * ac.one_minus_b1;
   v = v * ac.b2 + ac.one_minus_b2 * g * g;

@@ -9,18 +9,17 @@ exchanges, all tiny next to the compute:
   2. seam reduce of the image gradient: the contributions a rank computed for its halo rows are added to the
      neighbour's own rows (<= 2 x APRON x W x 3 floats),
   3. halo refresh of the updated image rows.
-Default ("peer" mode): all three run INSIDE the library, as kernels that read the peers' mailboxes over NVLink (CUDA
-IPC peer memory, csrc/comm.cu), so an iteration is one CUDA graph per rank -- `stb_iterate_banded`.  Fallback ("nccl"
-mode, `STB_COMM=nccl` or when the peer mapping cannot be set up): the host drives `stb_iterate_fwd` -> NCCL all-reduce
--> `stb_iterate_bwd` -> NCCL send/recv -> `stb_adam_update` (exchange_add_grad / exchange_halo below).
+All three run INSIDE the library, as kernels that read the peers' mailboxes over NVLink (CUDA IPC peer memory,
+csrc/comm.cu), so an iteration is one CUDA graph per rank -- `stb_iterate_banded` / `stb_iterate_lbfgs_banded`.  When
+the ranks cannot map each other's memory, the scales are not tiled: every rank runs the whole image.
 The reference's own multi-device call, `StyleTransfer(devices=[a, b])` (a 2-GPU layer split, ST:326-333), runs this
 tiling instead: one rank per listed device, as threads of the calling process (StyleTransfer._stylize_devices), with
 the exchanges inside the library.
 
 Collectives that are per SCALE, not per iteration (mailbox handle exchange, barriers, tiled style statistics, the
-final gather of the bands) go through a small group interface: `TorchGroup` (torch.distributed, one process per GPU)
-or `ThreadGroup` (the ranks are threads of one process, each with its own device or all on one -- the two-device
-`StyleTransfer`, and how the test-suite runs the very same tiled path on a single-GPU box).
+final gather of the bands) go through a small group interface: `TorchGroup` (torch.distributed, one process per GPU;
+NCCL carries only these) or `ThreadGroup` (the ranks are threads of one process, each with its own device or all on
+one -- the two-device `StyleTransfer`, and how the test-suite runs the very same tiled path on a single-GPU box).
 """
 from __future__ import annotations
 
@@ -169,58 +168,6 @@ def default_group():
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
         return TorchGroup()
     return None
-
-
-# ------------------------------------------------------------------------------------------------ nccl-mode exchanges
-def _p2p(ops, group):
-    if ops:
-        for req in dist.batch_isend_irecv(ops):
-            req.wait()
-
-
-def exchange_add_grad(grad: torch.Tensor, band: Band, group=None):
-    """grad: [1,3,h_local,W] d loss/d(local image).  Adds the neighbours' halo contributions to this rank's own rows
-    (in place) and ships this rank's halo contributions to the neighbours."""
-    ops, recv = [], []
-    up, down = band.rank - 1, band.rank + 1
-    if band.top_apron > 0:  # my top apron = bottom own rows of `up`; `up`'s bottom apron = my first own rows
-        send = grad[:, :, :band.top_apron].contiguous()
-        n = min(APRON, band.own_rows)
-        buf = torch.empty_like(grad[:, :, band.own0:band.own0 + n])
-        ops += [dist.P2POp(dist.isend, send, up, group), dist.P2POp(dist.irecv, buf, up, group)]
-        recv.append((buf, band.own0, band.own0 + n))
-    if band.bottom_apron > 0:
-        end = band.own0 + band.own_rows
-        send = grad[:, :, end:end + band.bottom_apron].contiguous()
-        n = min(APRON, band.own_rows)
-        buf = torch.empty_like(grad[:, :, end - n:end])
-        ops += [dist.P2POp(dist.isend, send, down, group), dist.P2POp(dist.irecv, buf, down, group)]
-        recv.append((buf, end - n, end))
-    _p2p(ops, group)
-    for buf, lo, hi in recv:
-        grad[:, :, lo:hi] += buf
-    return grad
-
-
-def exchange_halo(x: torch.Tensor, band: Band, group=None):
-    """x: [1,C,h_local,W] whose own rows are current: refresh the apron rows from the neighbours' own rows (in place)."""
-    ops, recv = [], []
-    up, down = band.rank - 1, band.rank + 1
-    if band.top_apron > 0:
-        send = x[:, :, band.own0:band.own0 + APRON].contiguous()          # what `up` keeps as its bottom apron
-        buf = torch.empty_like(x[:, :, :band.top_apron])
-        ops += [dist.P2POp(dist.isend, send, up, group), dist.P2POp(dist.irecv, buf, up, group)]
-        recv.append((buf, 0, band.top_apron))
-    if band.bottom_apron > 0:
-        end = band.own0 + band.own_rows
-        send = x[:, :, end - APRON:end].contiguous()
-        buf = torch.empty_like(x[:, :, end:end + band.bottom_apron])
-        ops += [dist.P2POp(dist.isend, send, down, group), dist.P2POp(dist.irecv, buf, down, group)]
-        recv.append((buf, end, end + band.bottom_apron))
-    _p2p(ops, group)
-    for buf, lo, hi in recv:
-        x[:, :, lo:hi] = buf
-    return x
 
 
 # ------------------------------------------------------------------------------------------------ per-scale helpers

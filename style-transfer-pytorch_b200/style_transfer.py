@@ -340,25 +340,11 @@ class NativeVGG:
     def set_band(self, enabled, h_global=0, own_row0=0, own_rows=0):
         _lib.check(self.lib.stb_set_band(self.ctx, int(enabled), h_global, own_row0, own_rows))
 
-    def stats_view(self, h, w):
-        """fp32 tensor aliasing the stats block inside the workspace (what the ranks all-reduce)."""
-        p = ctypes.c_void_p()
-        n = ctypes.c_size_t()
-        _lib.check(self.lib.stb_stats_block(self.ctx, h, w, ctypes.byref(p), ctypes.byref(n)))
-        off = p.value - self._ws.data_ptr()
-        return self._ws[off:off + 4 * n.value].view(torch.float32)
-
     def iterate_fwd(self, image):
         _lib.check(self.lib.stb_iterate_fwd(self.ctx, _lib.ptr(image), _lib.cur_stream()))
 
     def iterate_bwd(self, image, grad, loss_host):
         _lib.check(self.lib.stb_iterate_bwd(self.ctx, _lib.ptr(image), _lib.ptr(grad), _lib.ptr(loss_host),
-                                            _lib.cur_stream()))
-
-    def adam_update(self, image, grad, exp_avg, exp_avg_sq, ema, row0, rows, step, lr, avg_decay):
-        _, _, h, w = image.shape
-        _lib.check(self.lib.stb_adam_update(_lib.ptr(image), _lib.ptr(grad), _lib.ptr(exp_avg), _lib.ptr(exp_avg_sq),
-                                            _lib.ptr(ema), h, w, row0, rows, step, lr, 0.9, 0.99, 1e-8, avg_decay,
                                             _lib.cur_stream()))
 
     # ------------------------------------------------------------------ peer-memory exchange (csrc/comm.cu)
@@ -630,7 +616,9 @@ class StyleTransfer:
         self._dist = self._group is not None and self._group.world > 1
         self._rank = self._group.rank if self._dist else 0
         self._world = self._group.world if self._dist else 1
-        self._comm_mode = os.environ.get('STB_COMM', 'peer')   # 'peer': exchanges inside the library; 'nccl': host-driven
+        # 'peer': tiled scales iterate with the exchanges inside the library; 'off': the ranks could not map each
+        # other's memory, so every scale runs replicated
+        self._comm_mode = 'peer'
         # 'halo': a band computes its own rows only and pulls one boundary row per layer from its neighbours (their
         # workspaces are mapped); 'apron': it recomputes 80-row aprons instead (no per-layer exchange); 'auto' (default):
         # per scale, halo rows when the image is at least HALO_MIN_WIDTH wide.  Measured (DESIGN.md section 6): the ~28
@@ -727,20 +715,12 @@ class StyleTransfer:
         self.average.note_update()
 
     def _iterate_banded(self, band, stats, grad, exp_avg, exp_avg_sq, step, lr, avg_decay):
-        """One iteration of a spatially tiled scale.  'peer' mode: one library call = one CUDA graph holding the
-        compute AND the three exchanges (kernels reading the peers' mailboxes over NVLink, csrc/comm.cu).  'nccl' mode
-        (fallback): the host drives the phases and NCCL moves the data."""
-        m = self.model
-        if self._comm_mode == 'peer':
-            m.iterate_banded(self.image, exp_avg, exp_avg_sq, self.average.value, step, lr, avg_decay, self._loss_host)
-        else:
-            m.iterate_fwd(self.image)
-            torch.distributed.all_reduce(stats)             # Gram sums, channel sums, content SSE, TV sum
-            m.iterate_bwd(self.image, grad, self._loss_host)
-            D.exchange_add_grad(grad, band)                 # seam reduce of the image gradient
-            m.adam_update(self.image, grad, exp_avg, exp_avg_sq, self.average.value, band.own0, band.own_rows, step,
-                          lr, avg_decay)
-            D.exchange_halo(self.image, band)               # refresh the halo rows of the iterate
+        """One iteration of a spatially tiled scale: one library call = one CUDA graph holding the compute AND the
+        three exchanges (kernels reading the peers' mailboxes over NVLink, csrc/comm.cu)."""
+        # band, stats and grad are unused: the library holds the band geometry, the statistics block and the gradient.
+        # They stay in the signature because bench.py calls this positionally.
+        self.model.iterate_banded(self.image, exp_avg, exp_avg_sq, self.average.value, step, lr, avg_decay,
+                                  self._loss_host)
         self.average.note_update()
 
     def _ensure_peer_memory(self, ws_sizes, cap_h, cap_w):
@@ -777,9 +757,9 @@ class StyleTransfer:
             elif self._sync is not None:    # in-process ranks have no NCCL: the driver runs the job untiled
                 raise _PeerUnavailable(err)
             else:
-                warnings.warn(f'peer-memory exchange unavailable on some rank ({err}); falling back to host-driven '
-                              'NCCL exchanges')
-                self._comm_mode = 'nccl'
+                warnings.warn(f'peer-memory exchange unavailable on some rank ({err}); running the tiled scales '
+                              'replicated')
+                self._comm_mode = 'off'
         if self._comm_mode != 'peer' or self._tile_mode == 'apron' or not self._wants_halo(cap_w):
             return
         need = max(m.workspace_bytes(h, w) for h, w in ws_sizes) + 4096
@@ -823,8 +803,6 @@ class StyleTransfer:
         """Per tiled scale (collective): zero the iteration stamps between two barriers, hand the band geometry to the
         library."""
         g, m = self._group, self.model
-        if self._comm_mode != 'peer':
-            return
         bands = D.all_bands(band.H, self._world)
         g.barrier()
         m.comm_reset()
@@ -1073,11 +1051,9 @@ class StyleTransfer:
                     else:
                         sw, sh = size_to_fit(simg.size, style_size)
                     styles.append((sw, sh, src))
-                # multi-GPU: tile this scale into horizontal bands (None: too small, every rank runs the whole image).
-                # L-BFGS is tiled only with the exchanges inside the library ('peer'): its step needs 22 cross-rank
-                # reductions per iteration, which run as kernels in the iteration's graph.  Under host-driven NCCL
-                # exchanges every rank runs the whole image.
-                tiled = self._dist and (optimizer == 'adam' or self._comm_mode == 'peer')
+                # multi-GPU: tile this scale into horizontal bands (None: too small, or the ranks cannot map each
+                # other's memory: every rank runs the whole image)
+                tiled = self._dist and self._comm_mode == 'peer'
                 band = D.make_band(ch, self._rank, self._world) if tiled else None
                 h_loc = band.h_local if band is not None else ch
                 self.model.set_band(False)
@@ -1100,7 +1076,7 @@ class StyleTransfer:
                         lb = D.make_band(lh, self._rank, self._world)
                         end_sizes.append((lb.h_local if lb is not None else lh, lw))
                     self._ensure_peer_memory([(h_loc, cw)] + style_sizes + end_sizes, max(cap_h, h_loc), max(ew, cw))
-                    if optimizer == 'lbfgs' and self._comm_mode != 'peer':   # the peer mapping failed on some rank
+                    if self._comm_mode != 'peer':   # the peer mapping failed on some rank
                         band, h_loc = None, ch
                 self.model.ensure_workspace([(h_loc, cw)] + style_sizes)
 
@@ -1143,13 +1119,8 @@ class StyleTransfer:
                     else:  # warm start at the new size, step counter carried over (ST:285-295, 460-462)
                         exp_avg = self.model.resize(exp_avg, (ch, cw), 'bicubic')
                         exp_avg_sq = self.model.resize(exp_avg_sq, (ch, cw), 'bilinear', 'relu')
-                    if band is not None:
-                        if exp_avg.shape[2] != h_loc:
-                            exp_avg, exp_avg_sq = D.local_slice(exp_avg, band), D.local_slice(exp_avg_sq, band)
-                        stats = grad = None
-                        if self._comm_mode != 'peer':   # host-driven exchanges need torch views of both
-                            stats = self.model.stats_view(h_loc, cw)
-                            grad = torch.empty_like(self.image)
+                    if band is not None and exp_avg.shape[2] != h_loc:
+                        exp_avg, exp_avg_sq = D.local_slice(exp_avg, band), D.local_slice(exp_avg_sq, band)
                 else:
                     lbfgs_state = None   # hand the previous scale's block back before the new one is allocated
                     lbfgs_state = self._lbfgs_state(band.own_rows if band is not None else ch, cw)
@@ -1162,7 +1133,7 @@ class StyleTransfer:
                         sync.before_launch(self, step + 1)
                     if optimizer == 'adam' and band is not None:
                         step += 1
-                        self._iterate_banded(band, stats, grad, exp_avg, exp_avg_sq, step, step_size, avg_decay)
+                        self._iterate_banded(band, None, None, exp_avg, exp_avg_sq, step, step_size, avg_decay)
                     elif optimizer == 'adam':
                         step += 1
                         self._iterate(exp_avg, exp_avg_sq, step, step_size, avg_decay, callback is not None)
@@ -1181,13 +1152,8 @@ class StyleTransfer:
                         for device in self.devices:
                             if device.type == 'cuda':
                                 gpu_ram = max(gpu_ram, torch.cuda.max_memory_allocated(device))
-                        if band is not None and self._comm_mode != 'peer':
-                            torch.cuda.current_stream().synchronize()   # host-driven exchanges: plain read-back
-                            n = self.model.n_terms
-                            self.last_loss_terms = (self._loss_host[:n].clone() if n <= 8
-                                                    else self.model.loss_terms())
-                        else:   # the reference syncs here (loss.item()); this waits for the loss only
-                            self.last_loss_terms = self._wait_loss(step)
+                        # the reference syncs here (loss.item()); this waits for the loss only
+                        self.last_loss_terms = self._wait_loss(step)
                         loss_value = float(self.last_loss_terms[0])
                         callback(STIterate(w=cw, h=ch, i=i, i_max=actual_its, loss=loss_value, time=time.time(),
                                            gpu_ram=gpu_ram))

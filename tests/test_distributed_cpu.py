@@ -1,27 +1,16 @@
-"""-m "not gpu": the multi-GPU band scheme on CPU with the gloo backend (world_size 2 and 3).
+"""-m "not gpu": the multi-GPU band scheme on CPU (2 and 3 bands), and the per-scale group collectives.
 
 A small translation-invariant network stands in for VGG (same structure of the problem: local conv/pool trunk,
-loss = function of GLOBAL pixel sums + a per-pixel term).  Each rank works on its band + aprons, the "stats" are
-all-reduced, gradients of the halo rows are exchanged and added, the image halo is refreshed -- exactly the host
-protocol around stb_iterate_fwd / stb_iterate_bwd / stb_adam_update -- and the result must equal the full-image run.
+loss = function of GLOBAL pixel sums + a per-pixel term).  Each band works on its own rows + aprons, the "stats" of the
+own rows are summed over the bands, the gradients of the apron rows are added to the neighbours' own rows, the image
+halo is refreshed -- the three exchanges of a tiled iteration -- and the result must equal the full-image run.
 """
-import os
-import socket
-
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 import torch.nn.functional as F
 
 import style_transfer_b200  # noqa: F401  (registers the package)
 from style_transfer_b200 import distributed as D
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(('127.0.0.1', 0))
-        return s.getsockname()[1]
 
 
 def _net(x, w1, w2, w3):
@@ -50,64 +39,47 @@ def _full_reference(x, target):
     return loss.item(), x.grad
 
 
-def _worker(rank, world, port, H, W, out):
-    os.environ.update(MASTER_ADDR='127.0.0.1', MASTER_PORT=str(port))
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-    try:
-        torch.manual_seed(1)
-        x_full = torch.rand(1, 3, H, W)
-        target = torch.linspace(0, 1, 6)[None]
-        band = D.make_band(H, rank, world)
-        assert band is not None
+@pytest.mark.parametrize('world,H', [(2, 256), (3, 400), (2, 211)])
+def test_band_exchanges_equal_full(world, H):
+    W = 40
+    torch.manual_seed(1)
+    x_full = torch.rand(1, 3, H, W)
+    target = torch.linspace(0, 1, 6)[None]
+    bands = D.all_bands(H, world)
+    assert all(b is not None for b in bands)
+    xs, stats_local, pix = [], [], []
+    for band in bands:
         x = D.local_slice(x_full, band).requires_grad_()
         f = _net(x, *_weights())
         lo, rows = band.own0 // 4, band.own_rows // 4
         if band.own_end == H:
             rows = f.shape[2] - lo
-        stats_local = f[:, :, lo:lo + rows].sum(dim=(2, 3))          # own rows only
-        stats = stats_local.detach().clone()
-        dist.all_reduce(stats)                                        # == the stats-block all-reduce
-        n_global = (H // 4) * (W // 4)
-        g_stats = 2 * (stats / n_global - target) / n_global          # d loss / d stats from the reduced statistics
-        own = slice(band.own0, band.own0 + band.own_rows)
-        pix = 0.1 * (x[:, :, own] ** 2).sum() / (3 * H * W)          # per-pixel term on own rows only
-        (stats_local * g_stats).sum().backward(retain_graph=True)
-        pix.backward()
-        grad = x.grad.clone()
-        D.exchange_add_grad(grad, band)                               # seam exchange
-        loss = ((stats / n_global - target) ** 2).sum()
-        pl = pix.detach().clone()
-        dist.all_reduce(pl)
-        loss = loss + pl
-        # "update" own rows, refresh the halo, gather
-        new = x.detach().clone()
+        xs.append(x)
+        stats_local.append(f[:, :, lo:lo + rows].sum(dim=(2, 3)))                        # own rows only
+        pix.append(0.1 * (x[:, :, band.own0:band.own0 + band.own_rows] ** 2).sum() / (3 * H * W))
+    stats = sum(s.detach() for s in stats_local)                      # == the stats-block all-reduce
+    n_global = (H // 4) * (W // 4)
+    g_stats = 2 * (stats / n_global - target) / n_global              # d loss / d stats from the reduced statistics
+    # seam add: each band's gradient goes to its rows of the full gradient, so its aprons' share lands on the
+    # neighbours' own rows
+    grad = torch.zeros_like(x_full)
+    for band, x, s, p in zip(bands, xs, stats_local, pix):
+        (s * g_stats).sum().backward()
+        p.backward()
+        grad[:, :, band.loc_begin:band.loc_end] += x.grad
+    loss = ((stats / n_global - target) ** 2).sum() + sum(p.detach() for p in pix)
+    # "update" the own rows of every band, then refresh the halos: each band's local rows read back from the full image
+    new = x_full.clone()
+    for band in bands:
+        own = slice(band.own_begin, band.own_end)
         new[:, :, own] -= 0.5 * grad[:, :, own]
-        D.exchange_halo(new, band)
-        full_new = D.gather_rows(new, band)
-        ref_loss, ref_grad = _full_reference(x_full, target)
-        ok = abs(loss.item() - ref_loss) < 1e-5 * max(1, abs(ref_loss))
-        ok &= torch.allclose(grad[:, :, own], ref_grad[:, :, band.own_begin:band.own_end], atol=1e-6, rtol=1e-4)
-        expect_new = x_full - 0.5 * ref_grad
-        ok &= torch.allclose(full_new, expect_new, atol=1e-6, rtol=1e-4)
-        ok &= torch.allclose(new, expect_new[:, :, band.loc_begin:band.loc_end], atol=1e-6, rtol=1e-4)  # halos refreshed
-        out[rank] = bool(ok)
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.parametrize('world,H', [(2, 256), (3, 400), (2, 211)])
-def test_banded_equals_full(world, H):
-    ctx = mp.get_context('spawn')
-    mgr = ctx.Manager()
-    out = mgr.dict()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, H, 40, out)) for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(120)
-        assert p.exitcode == 0
-    assert all(out.get(r) for r in range(world)), dict(out)
+    ref_loss, ref_grad = _full_reference(x_full, target)
+    assert abs(loss.item() - ref_loss) < 1e-5 * max(1, abs(ref_loss))
+    torch.testing.assert_close(grad, ref_grad, atol=1e-6, rtol=1e-4)
+    expect_new = x_full - 0.5 * ref_grad
+    for band in bands:
+        torch.testing.assert_close(D.local_slice(new, band), expect_new[:, :, band.loc_begin:band.loc_end],
+                                   atol=1e-6, rtol=1e-4)
 
 
 def test_band_geometry():

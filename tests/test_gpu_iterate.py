@@ -333,27 +333,6 @@ def test_graphed_iterations_equal_eager_ones(G, vgg_weights):
         torch.testing.assert_close(a, b, rtol=0, atol=0)
 
 
-def test_adam_update_rows_on_one_gpu(G):
-    """stb_adam_update (the optimiser of the host-driven multi-GPU mode) on a row window: rows outside stay untouched."""
-    from style_transfer_b200 import _lib
-    H, W, r0, rows = 40, 52, 16, 16
-    g = torch.Generator().manual_seed(5)
-    x, grad = torch.rand(1, 3, H, W, generator=g), torch.randn(1, 3, H, W, generator=g) * 1e-3
-    ea, eas, ema = torch.randn(1, 3, H, W, generator=g) * 1e-4, torch.rand(1, 3, H, W, generator=g) * 1e-8, x * 0.3
-    dev = [t.to(G.DEV).contiguous() for t in (x, grad, ea, eas, ema)]
-    _lib.check(_lib.load().stb_adam_update(_lib.ptr(dev[0]), _lib.ptr(dev[1]), _lib.ptr(dev[2]), _lib.ptr(dev[3]),
-                                           _lib.ptr(dev[4]), H, W, r0, rows, 9, 0.02, 0.9, 0.99, 1e-8, 0.99, _lib.cur_stream()))
-    torch.cuda.synchronize()
-    want = _adam_reference((x, ea, eas, ema), grad, 9)
-    sl = (slice(None), slice(None), slice(r0, r0 + rows))
-    for got, new, old in zip((dev[0], dev[2], dev[3], dev[4]), want, (x, ea, eas, ema)):
-        got = got.cpu()
-        assert (got[sl].double() - new[sl]).abs().max() <= 2e-6 * new.abs().max() + 1e-12
-        mask = torch.ones(H, dtype=torch.bool)
-        mask[r0:r0 + rows] = False
-        torch.testing.assert_close(got[:, :, mask], old[:, :, mask], rtol=0, atol=0)
-
-
 # ---------------------------------------------------------------------------------------------- SURVEY 8(f) rows
 def test_lbfgs_runs_on_the_native_closure(G, vgg_weights):
     """optimizer='lbfgs' (ST:464-465): torch's L-BFGS on the host, closure = stb_iterate_ex(apply_update=0).  The loss

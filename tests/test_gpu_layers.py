@@ -339,8 +339,8 @@ def test_explicit_default_table_is_bit_identical(vgg_weights, lbfgs):
 
 
 def _banded_phases(st, cimg, simg, set_default_layers, its=4):
-    """The host-driven phases of a band (stb_iterate_fwd / stb_iterate_bwd) on a band that owns every row: gradient and
-    loss terms of `its` graphed closures."""
+    """The two halves of a band's closure (stb_iterate_fwd / stb_iterate_bwd) on a band that owns every row: gradient
+    and loss terms of `its` graphed closures."""
     m = st.model
     H, W = cimg.shape[2:]
     if set_default_layers:

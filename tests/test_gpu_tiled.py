@@ -106,3 +106,30 @@ def test_tiled_pyramid_mixes_replicated_and_banded_scales(vgg_weights, monkeypat
     np.testing.assert_allclose(tr, tr_s, rtol=2e-3)   # trajectories: sign-like Adam steps amplify 1e-4 differences
     assert np.abs(img - img_s).mean() < 1.0
     np.testing.assert_array_equal(tiled[1][1], img)
+
+
+@pytest.mark.parametrize('optimizer', ['adam', 'lbfgs'])
+def test_tiled_run_without_peer_memory_runs_replicated(vgg_weights, monkeypatch, optimizer):
+    """When some rank cannot map the others' memory, every rank runs every scale untiled: the same loss trace and image
+    as the single-GPU run, bit for bit.  The mapping is tried once, at the first scale tall enough to tile (272 rows);
+    the style image (150 rows) is too short to band, so no statistics are split across the ranks either."""
+    from style_transfer_b200 import _lib
+    from style_transfer_b200.style_transfer import NativeVGG
+    create, calls = NativeVGG.comm_create, []
+
+    def comm_create(self, rank, *args):
+        calls.append(rank)
+        if rank == 1:
+            raise _lib.NativeError('no peer memory on rank 1')
+        return create(self, rank, *args)
+
+    monkeypatch.setattr(NativeVGG, 'comm_create', comm_create)
+    content, style = O.synth_image(1, 16, 288, 384), O.synth_image(2, 32, 200, 150)
+    kw = dict(min_scale=272, end_scale=384, iterations=3, initial_iterations=4, optimizer=optimizer)
+    tiled = run_tiled(2, content, style, vgg_weights, kw)
+    tr_s, img_s = run_single(content, style, vgg_weights, kw)
+    assert sorted(calls) == [0, 1]
+    for tr, img, mode, _ in tiled:
+        assert mode == ('off', 'apron')
+        np.testing.assert_array_equal(tr, tr_s)
+        np.testing.assert_array_equal(img, img_s)

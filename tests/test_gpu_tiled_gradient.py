@@ -13,7 +13,7 @@ mode, floor-mode pooling on a ragged bottom band) against exact expectations:
 The ranks run as threads on one GPU (distributed.ThreadGroup, mailboxes and halo-mode workspaces connected with plain
 device pointers), as in test_gpu_lbfgs_tiled.py.
 
-Measured on an NVIDIA H100 80GB HBM3 (400 W limit) over the 12 cases of test_tiled_gradient_matches_the_untiled_closure
+Measured on an NVIDIA H100 80GB HBM3 (400 W limit) over the 12 cases of test_tiled_iteration_matches_the_untiled_closure
 (the whole file runs in ~15 s there):
   - halo mode: every own row of the tiled gradient equals g_ref bit for bit, in all six geometries.
   - apron mode: every own row at least APRON = 80 rows from every seam equals g_ref bit for bit (the backward receptive
@@ -27,11 +27,11 @@ Measured on an NVIDIA H100 80GB HBM3 (400 W limit) over the 12 cases of test_til
     sum): at most 3.8e-7 relative (fp32 summation order).  Bar 1.5e-6.  A row missing from a band is ~1/rows of a
     segment.
   - Adam on a band vs the float64 reference fed the gradient read back from the L-BFGS state: 8.7e-7 (bar 2e-6, as
-    tests/test_gpu_iterate.py); the host-driven mode's stb_adam_update vs the peer-mode update: 1.5e-7.
+    tests/test_gpu_iterate.py).
 Hand-made mutations (not committed), each of which made this file fail:
   1. no lower-neighbour seam add (has_dn = false in adam_seam_kernel and lbfgs_seam_gather_kernel): the apron-mode seam
      bars fail in all six geometries, per row 0.40 ... 0.48 (bar 6e-3), per zone 0.26 ... 0.34 (bar 5e-3); the
-     host-driven gradient no longer equals the peer one.
+     seam sum restated in torch (case (e)) no longer equals the peer-mode gradient.
   2. the backward pass's halo exchanges publish their stamps but copy no row: the halo-mode bit identity fails in all
      six geometries, max |g - g_ref| / max |g_ref| 0.29 ... 0.52.
   3. band_rows gives a bottom band with own rows below local row 0 one row fewer at the pooled levels: the statistics
@@ -296,11 +296,11 @@ def _run_ranks(job, world, halo):
     return bands, _threads(world, rank_fn)
 
 
-def _host_driven_gradients(job, bands, ranks):
-    """(e) The library half of the host-driven (STB_COMM=nccl) mode, in one thread and without communication: per band
+def _host_seam_gradients(job, bands, ranks):
+    """(e) An independent restatement of the apron-mode seam sum, in one thread and without communication: per band
     stb_iterate_fwd, the statistics blocks summed on the device in rank order (ThreadGroup.all_reduce_sum),
-    stb_iterate_bwd, then the seams added as distributed.exchange_add_grad does (own, upper neighbour's bottom apron,
-    lower neighbour's top apron).  Returns the full local gradients [1,3,h_local,W]."""
+    stb_iterate_bwd, then the seams added in torch (own, upper neighbour's bottom apron, lower neighbour's top apron).
+    Returns the full local gradients [1,3,h_local,W]."""
     W = job.W
     x0s = [D.local_slice(job.img, b) for b in bands]
     views = [_stats_block(r['m'], b.h_local, W) for b, r in zip(bands, ranks)]
@@ -348,9 +348,9 @@ def _row_metric(g, ref):
 
 @pytest.mark.parametrize('mode', ['apron', 'halo'])
 @pytest.mark.parametrize('world,H,W', GEOMS)
-def test_tiled_gradient_matches_the_untiled_closure(vgg_weights, world, H, W, mode):
-    """(b) statistics, (c) closure gradient and loss terms, (d) Adam on a band, (e, apron mode) the host-driven mode's
-    library half -- see the module docstring for R and g_ref."""
+def test_tiled_iteration_matches_the_untiled_closure(vgg_weights, world, H, W, mode):
+    """(b) statistics, (c) closure gradient and loss terms, (d) Adam on a band, (e, apron mode) the seam sum restated
+    on the host -- see the module docstring for R and g_ref."""
     halo = mode == 'halo'
     job = _job(vgg_weights, H, W)
     job.set_band(True)
@@ -392,20 +392,11 @@ def test_tiled_gradient_matches_the_untiled_closure(vgg_weights, world, H, W, mo
             adam_err = max(adam_err, (got[:, own].double() - w).abs().max().item() / max(w.abs().max().item(), 1e-30))
     metrics['adam_rel_max'] = adam_err
 
-    # (e) apron mode: the host-driven mode's library half gives the peer-mode gradient and Adam step
+    # (e) apron mode: the seam sum restated on the host gives the peer-mode gradient
     if not halo:
-        host = _host_driven_gradients(job, bands, ranks)
-        host_equal, host_adam = True, 0.0
-        for b, r, gl in zip(bands, ranks, host):
-            own = slice(b.own0, b.own0 + b.own_rows)
-            host_equal = host_equal and torch.equal(gl[0, :, own].cpu(), r['g'])
-            x, ea = D.local_slice(job.img, b), D.local_slice(job.exp_avg, b)
-            eas, ema = D.local_slice(job.exp_avg_sq, b), D.local_slice(job.img, b) * 0.01
-            r['m'].adam_update(x, gl, ea, eas, ema, b.own0, b.own_rows, FIRST_STEP, LR, 0.99)
-            torch.cuda.synchronize()
-            for got, w in zip((x, ea, eas, ema), r['after1']):
-                host_adam = max(host_adam, _rel(got[0, :, own].cpu(), w[:, own]))
-        metrics['host_grad_equal'], metrics['host_adam_rel_max'] = host_equal, host_adam
+        host = _host_seam_gradients(job, bands, ranks)
+        metrics['host_grad_equal'] = all(torch.equal(gl[0, :, b.own0:b.own0 + b.own_rows].cpu(), r['g'])
+                                         for b, r, gl in zip(bands, ranks, host))
     print('METRICS', metrics)
 
     # (b)
@@ -443,4 +434,3 @@ def test_tiled_gradient_matches_the_untiled_closure(vgg_weights, world, H, W, mo
     # (e)
     if not halo:
         assert metrics['host_grad_equal'], metrics
-        assert metrics['host_adam_rel_max'] <= ADAM_BAR, metrics
